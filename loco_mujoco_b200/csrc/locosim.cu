@@ -3,6 +3,8 @@
 // One fused kernel per control step: load state (HBM, env-major, coalesced per warp) -> n_substeps x
 // [kinematics, CRB, collision, constraint assembly, Newton solve, integrate] entirely in shared memory ->
 // observation gather + has_fallen + reward -> in-kernel auto-reset from the trajectory table -> store.
+// Or (LOCOSIM_RESORT, default for UnitreeA1) the same step as several launches over ranges of sub-steps, with the envs
+// regrouped by solver effort between launches (substep_kernel).
 // See locosim_core.cuh for the per-warp algorithm and DESIGN.md for the layout / roofline accounting.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -100,6 +102,63 @@ __global__ void reset_kernel(int ms, DevTask t, EngineState st, const uint8_t* m
     st.dr_row[env] = prow;
     st.cursor[env] = tr * t.traj_len + sp;
   }
+}
+
+// ----------------------------------------------------------------------------------------------------------
+// Sub-step launches (LOCOSIM_RESORT = S < n_substeps): the control step runs as ceil(n_substeps / S) launches of the step
+// kernel, each over sub-steps [k0, k1), and the envs are regrouped by solver effort between launches. Consecutive sub-steps
+// of an env cost alike (the lock-step cost of a block follows its hardest env sub-step by sub-step), the next control step
+// under random actions much less so. What the fused kernel keeps in shared memory across sub-steps is carried in HBM
+// (SplitState::carry); qpos / qvel / qacc_warmstart are stored as at the end of a step. Every launch appends its envs to
+// per-key buckets and the next launch takes its envs from them, hardest first, so that regrouping needs no extra launch.
+// ----------------------------------------------------------------------------------------------------------
+#define LS_RANK_BUCKETS 128
+#define LS_CARRY 32       // words per env: iter_sum, mpr_calls, sep_next, reward, sep_pair[4], sep_dir[4][3], grf[12]
+struct SplitState {
+  int* carry;             // [N, LS_CARRY]
+  int* bcount;            // [2, LS_RANK_BUCKETS] envs per key bucket: read by one launch, appended to by the other
+  int* benv;              // [2, LS_RANK_BUCKETS, N] the envs of every bucket (a permutation of all envs)
+  int* seq;               // [2] buffer read by the current launch, blocks of the current launch that have finished
+  int regroup, key_shift;
+};
+
+// env of position `pos` of the descending key order of the buckets (called by the whole warp)
+__device__ __forceinline__ int bucket_env(const int* __restrict__ cnt, const int* __restrict__ benv, int n_envs, int pos) {
+  const int lane = threadIdx.x & 31;
+  int c[4], s = 0;
+#pragma unroll
+  for (int j = 0; j < 4; j++) { c[j] = cnt[LS_RANK_BUCKETS - 1 - 4 * lane - j]; s += c[j]; }
+  int incl = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+  const int src = __ffs(__ballot_sync(0xffffffffu, incl > pos)) - 1;
+  int b = 0, off = 0;
+  if (lane == src) {
+    int acc = incl - s;
+    bool found = false;
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      if (!found && pos < acc + c[j]) { b = LS_RANK_BUCKETS - 1 - 4 * lane - j; off = pos - acc; found = true; }
+      acc += c[j];
+    }
+  }
+  b = __shfl_sync(0xffffffffu, b, src); off = __shfl_sync(0xffffffffu, off, src);
+  return benv[(size_t)b * n_envs + off];
+}
+
+// regrouping key of a sub-step launch: key mode 3 of the fused kernel with the counts of this launch's sub-steps scaled to a
+// whole control step
+template <class C>
+__device__ __forceinline__ int launch_key(const DevTask& t, const EnvS<C>& e, int k0, int k1, int iter0, int mpr0,
+                                          int key_mode_in) {
+  const int ns = k1 - k0, mpr_w = (key_mode_in >> 8) & 255;
+  return (e.iter_sum - iter0) * t.n_substeps / ns + (e.nefc >> 1) + mpr_w * min((e.mpr_calls - mpr0) * t.n_substeps / ns, 64);
+}
+__device__ __forceinline__ void append_env(const SplitState& split, int wr, int env, int n_envs, int key) {
+  key >>= split.key_shift;
+  const int b = key < LS_RANK_BUCKETS - 1 ? key : LS_RANK_BUCKETS - 1;
+  const int pos = atomicAdd(&split.bcount[wr * LS_RANK_BUCKETS + b], 1);
+  split.benv[((size_t)wr * LS_RANK_BUCKETS + b) * n_envs + pos] = env;
 }
 
 // ----------------------------------------------------------------------------------------------------------
@@ -273,12 +332,249 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// sub-step kernel body: the fused step kernel above restricted to sub-steps [k0, k1) of the control step.
+// It repeats step_kernel's staging, load, reward and epilogue on purpose: folding both into one template (or into shared
+// inline helpers) changes the code nvcc 12.9 generates for the fused kernel (sm_90a: 272 -> 260 bytes of spill stores for
+// CfgEllEuler), which is the path of every configuration that does not split. A change to one epilogue must be made to both;
+// tests/test_substep_launches.py holds them to the same bits (A1, HumanoidTorque, Talos with DR, foot forces,
+// the tracking reward, ghost warps).
+// ----------------------------------------------------------------------------------------------------------
+template <class C>
+__device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, DevTask t, SolverOpts so, EngineState st,
+                                             const float* __restrict__ action, float* __restrict__ obs,
+                                             float* __restrict__ reward, uint8_t* __restrict__ done,
+                                             float* __restrict__ next_obs, int n_envs, int auto_reset, uint64_t seed,
+                                             int64_t env_off, int sync_substeps, int key_mode_in,
+                                             const unsigned char* __restrict__ stage_src, int stage_bytes, int k0, int k1,
+                                             SplitState split) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int key_mode = key_mode_in & 0xffff;
+  if (stage_bytes > 0) {
+    // LOCOSIM_STAGE (default on where it fits): the table of the PRIMITIVE candidate pairs of the mid-phase (packed geom pair +
+    // bound; UnitreeA1: 357 entries read in every dynamics evaluation by every warp) is staged once per block into the shared
+    // memory behind the per-env working sets by ONE TMA bulk copy (cp.async.bulk global -> shared::cta, completion on an
+    // mbarrier); EnvS::pk_tab points to it, DevModel::pk_n is its entry count.
+    unsigned char* dst = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
+    const unsigned dst_a = (unsigned)__cvta_generic_to_shared(dst);
+    const unsigned bar_a = dst_a + (unsigned)stage_bytes;
+    if (threadIdx.x == 0) {
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"((unsigned)stage_bytes) : "memory");
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
+                   "l"(stage_src), "r"((unsigned)stage_bytes), "r"(bar_a)
+                   : "memory");
+    }
+    __syncthreads();                                    // (the barrier object is initialised before anybody polls it)
+    unsigned ok = 0;
+    while (!ok)
+      asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                   : "=r"(ok) : "r"(bar_a) : "memory");
+  }
+  // warps past the last env shadow it (same barriers, no stores): the block-wide barriers inside the solver have
+  // data-dependent counts, so every warp of a block has to run the physics
+  const int slot_raw = blockIdx.x * (blockDim.x >> 5) + warp;
+  const bool ghost = slot_raw >= n_envs;
+  const int slot = ghost ? n_envs - 1 : slot_raw;
+  const int rd = split.seq[0] & 1;      // bucket buffer this launch reads; it appends to the other one
+  const int env = split.regroup ? bucket_env(split.bcount + rd * LS_RANK_BUCKETS,
+                                             split.benv + (size_t)rd * LS_RANK_BUCKETS * n_envs, n_envs, slot)
+                                : slot;
+  EnvS<C>& e = reinterpret_cast<EnvS<C>*>(smem_raw)[warp];
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv, nu = m.nu, D = t.obs_dim;
+  if (lane == 0) {
+    e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
+    if (stage_bytes > 0) {
+      const unsigned char* sm = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
+      e.pk_tab = reinterpret_cast<const int*>(sm);
+    } else { e.pk_tab = m.pair_packed; }
+  }
+
+  // ---- load state ----
+  for (int i = lane; i < nv; i += 32) {
+    e.qpos[i] = st.qpos[(size_t)env * nv + i];
+    e.qvel[i] = st.qvel[(size_t)env * nv + i];
+    e.qacc_ws[i] = st.ws[(size_t)env * nv + i];
+    e.qacc[i] = 0;
+  }
+  for (int i = lane; i < nu; i += 32) e.ctrl[t.act_idx[i]] = action[(size_t)env * nu + i] * t.act_delta[i] + t.act_mean[i];
+  if (lane < 4) e.goal[lane] = st.goal[(size_t)env * 4 + lane];
+  __syncwarp();
+  init_workspace(ms, e);
+  float rew = 0;
+  int* carry = split.carry + (size_t)env * LS_CARRY;
+  static_assert(EnvS<C>::NSEP <= 4 && 3 * LS_MAX_GRF <= 12, "carry record layout");
+  if (k0 > 0) {
+    // what the previous launches of this control step left behind (init_workspace above cleared part of it)
+    if (lane == 0) { e.iter_sum = carry[0]; e.mpr_calls = carry[1]; e.sep_next = carry[2]; rew = __int_as_float(carry[3]); }
+    if (lane < EnvS<C>::NSEP) e.sep_pair[lane] = carry[4 + lane];
+    if (lane < 3 * EnvS<C>::NSEP) (&e.sep_dir[0][0])[lane] = __int_as_float(carry[8 + lane]);
+    if (lane < 3 * LS_MAX_GRF) e.grf[lane] = __int_as_float(carry[20 + lane]);
+    __syncwarp();
+  } else {
+    if (lane == 0) e.iter_sum = 0;
+    if (lane < 3 * LS_MAX_GRF) e.grf[lane] = 0;
+    // reward depends on the *previous* observation only (utils/reward.py via base.py:170-176): evaluate it now
+    if (t.reward_type == LS_REWARD_TARGET_VELOCITY) { float d = obs_value(t, e, t.ri[0]) - t.rp[0]; rew = expf(-d * d); }
+    else if (t.reward_type == LS_REWARD_VELOCITY_VECTOR) {
+      float g = obs_value(t, e, t.ri[3]);
+      float dx = obs_value(t, e, t.ri[0]) - g * obs_value(t, e, t.ri[2]);
+      float dy = obs_value(t, e, t.ri[1]) - g * obs_value(t, e, t.ri[2] + 1);
+      rew = expf(-5.0f * sqrtf(dx * dx + dy * dy));
+    } else if (t.reward_type == LS_REWARD_POS) rew = obs_value(t, e, t.ri[0]);
+  }
+  const int iter0 = e.iter_sum, mpr0 = e.mpr_calls;    // (the regrouping key counts this launch's sub-steps)
+
+  // ---- physics ----
+  if (sync_substeps) {
+    // keep the warps of a block in the same phase: they then share instruction-cache lines
+    for (int k = k0; k < k1; k++) { if (k % sync_substeps == 0) __syncthreads(); physics_substeps(ms, e, so, 1, t.grf_group, t.n_grf); }
+  } else {
+    physics_substeps(ms, e, so, k1 - k0, t.grf_group, t.n_grf);
+  }
+
+  if (k1 < t.n_substeps) {
+    // ---- not the last launch of the control step: state and carried fields to HBM, env into its bucket ----
+    if (!ghost) {
+      for (int i = lane; i < nv; i += 32) {
+        st.qpos[(size_t)env * nv + i] = e.qpos[i];
+        st.qvel[(size_t)env * nv + i] = e.qvel[i];
+        st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
+      }
+      if (lane == 0) { carry[0] = e.iter_sum; carry[1] = e.mpr_calls; carry[2] = e.sep_next; carry[3] = __float_as_int(rew); }
+      if (lane < EnvS<C>::NSEP) carry[4 + lane] = e.sep_pair[lane];
+      if (lane < 3 * EnvS<C>::NSEP) carry[8 + lane] = __float_as_int((&e.sep_dir[0][0])[lane]);
+      if (lane < 3 * LS_MAX_GRF) carry[20 + lane] = __float_as_int(e.grf[lane]);
+      if (lane == 0 && split.regroup) append_env(split, rd ^ 1, env, n_envs, launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in));
+    }
+    return;
+  }
+  if (ghost) return;
+
+  // ---- observation, termination, reward ----
+  bool bad = false;
+  for (int i = lane; i < nv; i += 32) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+  bool fallen = false;
+  for (int k = lane; k < t.n_done; k += 32) {
+    float v = obs_value(t, e, t.done_obs_idx[k]);
+    fallen |= (v < t.done_lo[k]) || (v > t.done_hi[k]);
+  }
+  bad = __any_sync(0xffffffffu, bad);
+  fallen = __any_sync(0xffffffffu, fallen) && t.use_absorbing;
+  const bool is_done = fallen || bad;
+  if (t.reward_type == LS_REWARD_TRACKING) {
+    // mocap-tracking reward (include/locosim_task.h): the cursor advances one sample, the observation reached by this step
+    // is compared with the table row at the advanced cursor
+    int cur = st.cursor[env];
+    const int tj = cur / t.traj_len;
+    int sp = cur - tj * t.traj_len;
+    sp = sp + 1 < t.traj_len ? sp + 1 : t.traj_len - 1;
+    cur = tj * t.traj_len + sp;
+    const float* ref = t.table + (size_t)cur * (2 * nv + t.n_goal);
+    float ep = 0, ev = 0;
+    for (int k = lane; k < D; k += 32) {
+      const int ty = t.obs_src_type[k], idx = t.obs_src_idx[k];
+      if (ty == LS_OBS_QPOS) { const float d = e.qpos[idx] - ref[idx]; ep += d * d; }
+      else if (ty == LS_OBS_QVEL) { const float d = e.qvel[idx] - ref[nv + idx]; ev += d * d; }
+    }
+    ep = warp_sum(ep); ev = warp_sum(ev);
+    rew = bad ? 0.0f : t.track[0] * expf(-t.track[1] * ep) + t.track[2] * expf(-t.track[3] * ev);
+    if (lane == 0) st.cursor[env] = cur;
+  }
+  for (int k = lane; k < D; k += 32) {
+    float v = obs_value(t, e, k);
+    if (bad) v = 0.0f;
+    obs[(size_t)env * D + k] = v;
+  }
+  if (lane == 0) {
+    float r = rew;
+    reward[env] = r;
+    done[env] = is_done ? 1 : 0;
+    int* cnt = st.counters + (size_t)env * 8;
+    cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
+    if (bad) cnt[4] += 1;
+    {
+      int key = e.iter_sum;
+      const int mpr_w = (key_mode >> 8) & 255;           // weight of one MPR run in Newton-iteration units
+      key_mode &= 255;
+      if (key_mode == 1) key = (cnt[5] + e.iter_sum + 1) >> 1;
+      else if (key_mode == 2) key = e.solver_iter * 8;
+      else if (key_mode == 3) key = e.iter_sum + (e.nefc >> 1) + mpr_w * min(e.mpr_calls, 64);
+      else if (key_mode == 4) key = (3 * cnt[5] + e.iter_sum + 2) >> 2;
+      else if (key_mode == 5) key = e.iter_sum + 4 * e.solver_iter;
+      else if (key_mode == 6) key = e.iter_sum + e.nefc;
+      else if (key_mode == 7) key = e.iter_sum + 4 * e.solver_iter + (e.nefc >> 1);
+      cnt[5] = key;
+    } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
+  }
+
+  // ---- auto-reset ----
+  if (is_done && (auto_reset || bad)) {
+    const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
+    int ep = st.episode[env];
+    int tr, sp;
+    draw_reset(seed, env_off + env, ep, t.n_traj, t.traj_len, &tr, &sp);
+    __syncwarp();
+    reset_env(ms, t, e, tr, sp, t.rot[0] >= 0 ? draw_rot_angle(seed, env_off + env, ep) : 0.0f);
+    if (lane == 0) {
+      const int prow = draw_pool_row(seed, env_off + env, ep, st.pool_K);
+      st.episode[env] = ep + 1; st.counters[(size_t)env * 8 + 1] += 1;
+      if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
+      st.dr_row[env] = prow;
+      st.cursor[env] = tr * t.traj_len + sp;
+      e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
+    }
+    __syncwarp();
+    for (int k = lane; k < t.n_goal; k += 32) st.goal[(size_t)env * 4 + k] = e.goal[k];
+  }
+  if (next_obs) for (int k = lane; k < D; k += 32) next_obs[(size_t)env * D + k] = obs_value(t, e, k);
+
+  // ---- store state ----
+  for (int i = lane; i < nv; i += 32) {
+    st.qpos[(size_t)env * nv + i] = e.qpos[i];
+    st.qvel[(size_t)env * nv + i] = e.qvel[i];
+    st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
+  }
+  if (lane == 0 && split.regroup) {
+    int key = launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in);
+    if (is_done && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
+    append_env(split, rd ^ 1, env, n_envs, key);
+  }
+}
+
+template <class C>
+__global__ void __launch_bounds__(512, 1) substep_kernel(int ms, DevTask t, SolverOpts so, EngineState st,
+                                                       const float* __restrict__ action, float* __restrict__ obs,
+                                                       float* __restrict__ reward, uint8_t* __restrict__ done,
+                                                       float* __restrict__ next_obs, int n_envs, int auto_reset,
+                                                       uint64_t seed, int64_t env_off, int sync_substeps, int key_mode_in,
+                                                       const unsigned char* __restrict__ stage_src, int stage_bytes, int k0,
+                                                       int k1, SplitState split) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  substep_body<C>(smem_raw, ms, t, so, st, action, obs, reward, done, next_obs, n_envs, auto_reset, seed, env_off,
+                     sync_substeps, key_mode_in, stage_src, stage_bytes, k0, k1, split);
+  // The block that finishes last (every other block has read its envs from the buckets by then) empties the buckets this
+  // launch read and hands the ones it filled to the next launch: no host-side launch counter, so CUDA graphs replay it.
+  __syncthreads();
+  int last = 0;
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last = atomicAdd(&split.seq[1], 1) == (int)gridDim.x - 1;
+  }
+  if (__syncthreads_or(last)) {
+    const int rd = split.seq[0] & 1;
+    for (int i = threadIdx.x; i < LS_RANK_BUCKETS; i += blockDim.x) split.bcount[rd * LS_RANK_BUCKETS + i] = 0;
+    if (threadIdx.x == 0) { split.seq[0] = rd ^ 1; split.seq[1] = 0; }
+  }
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // Regrouping: the warps of a block run the solver in lock-step, so a block is as slow as its hardest env. Solver effort
 // is strongly correlated from one control step to the next (lag-1 correlation of the per-step Newton iteration count
 // ~0.6), so before every step the envs are bucketed by the iteration count of their previous step (counting sort,
 // one block) and envs of similar effort share a block. Pure scheduling: results do not depend on the mapping.
 // ----------------------------------------------------------------------------------------------------------
-#define LS_RANK_BUCKETS 128
 __global__ void __launch_bounds__(1024) rank_kernel(const int* __restrict__ counters, int* __restrict__ perm, int n_envs,
                                                     int key_shift) {
   __shared__ int hist[LS_RANK_BUCKETS];
@@ -308,6 +604,8 @@ __global__ void __launch_bounds__(1024) rank_kernel(const int* __restrict__ coun
 struct locosim_handle {
   int device = 0, n_envs = 0, cfg = -1, wpb = 4, smem = 0, slot = -1, sync_substeps = 0, regroup = 1, key_shift = 0, key_mode = 3;
   int n_sm = 1;
+  int resort = 0;                   // sub-steps per launch of the step kernel (>= n_substeps: one fused launch per step)
+  SplitState split = {};
   uint64_t seed = 0;
   int64_t env_off = 0;
   HostModel hm;
@@ -347,10 +645,19 @@ template <class C>
 static int launch_step(locosim_handle* h, const float* a, float* o, float* r, uint8_t* d, float* no, int auto_reset,
                        cudaStream_t s) {
   int blocks = (h->n_envs + h->wpb - 1) / h->wpb;
-  if (h->regroup) rank_kernel<<<1, 1024, 0, s>>>(h->st.counters, h->st.perm, h->n_envs, h->key_shift);
-  step_kernel<C><<<blocks, h->wpb * 32, h->smem + (h->stage_bytes ? h->stage_bytes + 16 : 0), s>>>(
-      h->slot, h->dt, h->so, h->st, a, o, r, d, no, h->n_envs, auto_reset, h->seed, h->env_off, h->sync_substeps, h->key_mode,
-      h->d_stage, h->stage_bytes);
+  const int smem = h->smem + (h->stage_bytes ? h->stage_bytes + 16 : 0), nsub = h->dt.n_substeps;
+  if (h->resort >= nsub) {
+    if (h->regroup) rank_kernel<<<1, 1024, 0, s>>>(h->st.counters, h->st.perm, h->n_envs, h->key_shift);
+    step_kernel<C><<<blocks, h->wpb * 32, smem, s>>>(h->slot, h->dt, h->so, h->st, a, o, r, d, no, h->n_envs, auto_reset,
+                                                      h->seed, h->env_off, h->sync_substeps, h->key_mode, h->d_stage,
+                                                      h->stage_bytes);
+  } else {
+    for (int k0 = 0; k0 < nsub; k0 += h->resort)
+      substep_kernel<C><<<blocks, h->wpb * 32, smem, s>>>(h->slot, h->dt, h->so, h->st, a, o, r, d, no, h->n_envs, auto_reset,
+                                                         h->seed, h->env_off, h->sync_substeps, h->key_mode, h->d_stage,
+                                                         h->stage_bytes, k0, k0 + h->resort < nsub ? k0 + h->resort : nsub,
+                                                         h->split);
+  }
   CK(cudaGetLastError());
   return 0;
 }
@@ -402,6 +709,35 @@ static int setup_cfg(locosim_handle* h) {
     if (getenv("LOCOSIM_MPR_WEIGHT")) w = atoi(getenv("LOCOSIM_MPR_WEIGHT"));
     if (getenv("LOCOSIM_KEY_RESET")) kr = atoi(getenv("LOCOSIM_KEY_RESET")) + 1;
     h->key_mode = (h->key_mode & 255) | ((w & 255) << 8) | (kr << 16);
+  }
+  {
+    // sub-steps per launch (regrouping between launches), default by H100 A/B (bench.py, 4096 envs; fused = 10):
+    // UnitreeA1.simple 1.24 M env-steps/s fused, 1.31 M at 5, 1.33 M at 2, 1.28 M at 1 -> 2 for CfgEllEuler;
+    // HumanoidTorque.run (CfgPyrRK4) 0.437 M fused, 0.395 M at 5, 0.373 M at 2 -> fused. The configurations not measured
+    // (Talos / H1, G1) and batches that leave SMs without a full block (the spread geometry, MixedBatch members: config 4
+    // 0.76 M fused, 0.68 M at 2) keep the fused kernel.
+    const int nsub = h->dt.n_substeps;
+    const bool full = (h->n_envs + best - 1) / best >= h->n_sm;
+    h->resort = full && C::CONE == 1 && !C::RK4 ? 2 : nsub;
+    if (getenv("LOCOSIM_RESORT")) h->resort = atoi(getenv("LOCOSIM_RESORT"));
+    if (h->resort < 1 || h->resort > nsub) h->resort = nsub;
+    if (h->resort < nsub) {
+      const size_t N = (size_t)h->n_envs;
+      CK(cudaMalloc((void**)&h->split.carry, N * LS_CARRY * 4));
+      CK(cudaMalloc((void**)&h->split.bcount, 2 * LS_RANK_BUCKETS * 4));
+      CK(cudaMalloc((void**)&h->split.benv, 2 * LS_RANK_BUCKETS * N * 4));
+      CK(cudaMalloc((void**)&h->split.seq, 2 * 4));
+      CK(cudaMemset(h->split.carry, 0, N * LS_CARRY * 4));
+      CK(cudaMemset(h->split.bcount, 0, 2 * LS_RANK_BUCKETS * 4));
+      CK(cudaMemset(h->split.seq, 0, 2 * 4));
+      // the first launch reads buffer 0: every env in bucket 0, in env order (the identity mapping)
+      const int n = h->n_envs;
+      CK(cudaMemcpy(h->split.bcount, &n, 4, cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(h->split.benv, h->st.perm, N * 4, cudaMemcpyDeviceToDevice));
+      h->split.regroup = h->regroup;
+      h->split.key_shift = h->key_shift;
+      CK(cudaFuncSetAttribute(substep_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, dev_max));
+    }
   }
   h->so.sync_iters = 16;    // lock-step group = the whole block
   if (getenv("LOCOSIM_SYNC_ITERS")) { int v = atoi(getenv("LOCOSIM_SYNC_ITERS")); h->so.sync_iters = v == 1 ? 16 : v; }
@@ -513,6 +849,7 @@ void locosim_destroy(locosim_t* h) {
   cudaFree(h->st.qpos); cudaFree(h->st.qvel); cudaFree(h->st.ws); cudaFree(h->st.goal); cudaFree(h->st.episode);
   cudaFree(h->st.counters); cudaFree(h->st.dr_row); cudaFree(h->st.perm); cudaFree(h->st.cursor); cudaFree(h->d_pool);
   cudaFree(h->d_stage);
+  cudaFree(h->split.carry); cudaFree(h->split.bcount); cudaFree(h->split.benv); cudaFree(h->split.seq);
   delete h;
 }
 
@@ -657,7 +994,11 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
   return 0;
 }
 
-int locosim_kernels_per_step(const locosim_t* h) { return h->regroup ? 2 : 1; }
+int locosim_kernels_per_step(const locosim_t* h) {
+  const int nsub = h->dt.n_substeps;
+  if (h->resort < nsub) return (nsub + h->resort - 1) / h->resort;
+  return h->regroup ? 2 : 1;
+}
 int locosim_debug_counters(unsigned long long* out8) {
   return cudaMemcpyFromSymbol(out8, g_dbg, 64) == cudaSuccess ? 0 : 1;
 }

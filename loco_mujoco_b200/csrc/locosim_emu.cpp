@@ -24,6 +24,7 @@ struct EmuBase {
   virtual void contact(int k, double* o) = 0;
   virtual void grf(double* o, int clear) = 0;
   virtual void frames(double* gx, double* bx) = 0;
+  virtual void poison() = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -62,6 +63,25 @@ struct EmuT : EmuBase {
   void frames(double* gx, double* bx) override {
     for (int g = 0; g < m.ng; g++) for (int k = 0; k < 3; k++) gx[3 * g + k] = e.gxpos[g][k];
     for (int b = 0; b < m.nb; b++) { for (int k = 0; k < 3; k++) bx[7 * b + k] = e.xpos[b][k]; for (int k = 0; k < 4; k++) bx[7 * b + 3 + k] = e.xquat[b][k]; }
+  }
+  // What a sub-step launch of the CUDA engine (substep_kernel) starts from: the working set is lost except the fields it
+  // carries in HBM between launches (state, warm start, control, goal, the step's counters, the separating-direction cache,
+  // the summed foot forces); everything else is poisoned, then rebuilt the way the kernel rebuilds it.
+  void poison() override {
+    EnvS<C>* keep = new EnvS<C>(e);
+    memset((void*)&e, 0xff, sizeof(e));
+    for (int i = 0; i < m.nv; i++) { e.qpos[i] = keep->qpos[i]; e.qvel[i] = keep->qvel[i]; e.qacc_ws[i] = keep->qacc_ws[i]; e.qacc[i] = 0; }
+    for (int i = 0; i < m.nu; i++) e.ctrl[i] = keep->ctrl[i];
+    for (int k = 0; k < 4; k++) e.goal[k] = keep->goal[k];
+    e.prm = keep->prm; e.pk_tab = keep->pk_tab;
+    init_workspace(0, e);
+    e.iter_sum = keep->iter_sum; e.mpr_calls = keep->mpr_calls; e.sep_next = keep->sep_next;
+    for (int k = 0; k < EnvS<C>::NSEP; k++) {
+      e.sep_pair[k] = keep->sep_pair[k];
+      for (int j = 0; j < 3; j++) e.sep_dir[k][j] = keep->sep_dir[k][j];
+    }
+    for (int k = 0; k < 3 * LS_MAX_GRF; k++) e.grf[k] = keep->grf[k];
+    delete keep;
   }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
@@ -111,6 +131,7 @@ void emu_set_grf(EmuBase* s, const int* group, int ng, int n_grf) { s->grf_group
 void emu_get_grf(EmuBase* s, double* o, int clear) { s->grf(o, clear); }
 void emu_frames(EmuBase* s, double* gx, double* bx) { s->frames(gx, bx); }
 int emu_nefc(EmuBase* s) { return s->info(1); }
+void emu_poison(EmuBase* s) { s->poison(); }
 int emu_iter(EmuBase* s) { return s->info(2); }
 int emu_sizeof_env(int which) {
   switch (which) {
