@@ -104,7 +104,8 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
 int locosim_get_param_rows(locosim_t* h, int32_t* d_out, void* stream);
 
 /* Kernels enqueued by one locosim_step: the fused step kernel, preceded (default) by the one-block regrouping kernel that
- * buckets the envs by the solver effort of their previous step (scheduling only; results do not depend on it). */
+ * buckets the envs by the solver effort of their previous step (scheduling only; results do not depend on it); one per
+ * range of sub-steps with LOCOSIM_RESORT; 1 for the persistent sub-step kernel. */
 int locosim_kernels_per_step(const locosim_t* h);
 
 /* Measurement aid (bench.py): non-tensor FP32 FMA throughput of `device` in TFLOP/s, measured with a register-only
@@ -117,6 +118,12 @@ int locosim_debug_counters(unsigned long long* out8);
 
 /* Launch geometry chosen for this handle: warps(envs) per block, dynamic shared memory bytes per block, blocks. */
 int locosim_launch_info(const locosim_t* h, int* warps_per_block, int* smem_bytes, int* n_blocks);
+
+/* Measurement aid (tools/sm_timeline.py), persistent sub-step kernel only: every later step appends one record of 8 int64 per
+ * group to the device buffer d_records [1 + capacity, 8] (d_records[0] counts the records, zero it before the step): SM id,
+ * chunk, envs, pop start, group start, group end (%globaltimer, ns), Newton iterations summed over the envs, the largest of
+ * them. capacity 0 (or NULL) turns it off. Fails when the handle does not run the persistent kernel. */
+int locosim_set_timeline(locosim_t* h, long long* d_records, int capacity);
 
 #ifdef __cplusplus
 }

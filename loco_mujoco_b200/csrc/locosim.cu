@@ -4,7 +4,8 @@
 // [kinematics, CRB, collision, constraint assembly, Newton solve, integrate] entirely in shared memory ->
 // observation gather + has_fallen + reward -> in-kernel auto-reset from the trajectory table -> store.
 // Or (LOCOSIM_RESORT, default for UnitreeA1) the same step as several launches over ranges of sub-steps, with the envs
-// regrouped by solver effort between launches (substep_kernel).
+// regrouped by solver effort between launches (substep_kernel), or all of them in one persistent launch that regroups the
+// envs between chunks of sub-steps from a device-side queue (persist_kernel, default for UnitreeA1).
 // See locosim_core.cuh for the per-warp algorithm and DESIGN.md for the layout / roofline accounting.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -570,6 +571,403 @@ __global__ void __launch_bounds__(512, 1) substep_kernel(int ms, DevTask t, Solv
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// Persistent sub-step kernel (LOCOSIM_PERSIST, default where sub-step launches are): the whole control step in ONE launch
+// of min(SMs, blocks) blocks. The step is cut into chunks of LOCOSIM_RESORT sub-steps; the work unit is a group of up to
+// wpb envs running one chunk together. A warp that finishes a chunk of its env stores state and carry record and publishes
+// the env into the key bucket of the next chunk; a block pops its next group from the lowest chunk that has enough envs
+// ready, hardest keys first. So the envs are regrouped by the effort of their last chunk as in substep_kernel, but the
+// block prologue (TMA staging) is paid once per step and an SM that finishes early takes the next group instead of
+// idling in the wave tail of every launch.
+//
+// Memory ordering: an SM may hold a stale L1 line of an env it ran earlier in the same launch that another SM has since
+// advanced, so everything another block of this launch may have written (state, carry, env ids, counts) is read past L1
+// (ld.global.cg / ld.relaxed.gpu); publishing is a release: stores, __threadfence(), then the env id and the counts.
+// No grid barrier and no co-residency assumption: a block only waits for envs that running blocks hold, so the kernel
+// makes progress with any number of resident blocks.
+//
+// The body repeats substep_body on purpose (see the note there: folding changes the other kernels' code).
+// ----------------------------------------------------------------------------------------------------------
+#define LS_TL_WORDS 8     // timeline record: smid, chunk, envs, pop start, group start, group end (ns), iterations sum, max
+struct PersistQueue {
+  int* carry;             // [N, LS_CARRY] as SplitState::carry
+  int* cnt;               // [nch + 1, 3, LS_RANK_BUCKETS] per key bucket: slots reserved, envs published, envs taken
+  int* tot;               // [nch + 1, 2] per chunk: envs published, envs taken
+  int* benv;              // [nch + 1, LS_RANK_BUCKETS, N] env ids of the bucket slots, -1 = empty
+  int* seq;               // [2] parity of the step (which of the two chunk-0 sets it reads), blocks that have finished
+  long long* tl;          // optional timeline: [1 + tl_cap, LS_TL_WORDS], tl[0] = records written (NULL in the product path)
+  int tl_cap;
+  int nch, chunk, pool, regroup, key_shift;
+};
+// bucket set of chunk c: chunk 0 of this step and chunk 0 of the next (published by the last chunk) alternate between sets 0
+// and 1; chunks 1 .. nch-1 use sets 2 .. nch
+__device__ __forceinline__ int persist_set(int c, int nch, int par) { return c == 0 ? par : (c == nch ? par ^ 1 : c + 1); }
+__device__ __forceinline__ int ld_relaxed(const int* p) {
+  int v;
+  asm volatile("ld.relaxed.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_relaxed(int* p, int v) {
+  asm volatile("st.relaxed.gpu.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ long long global_ns() {
+  long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
+// publish `env` (lane 0; the warp's stores are fenced) into bucket `key` of chunk c
+__device__ __forceinline__ void persist_publish(const PersistQueue& q, int par, int c, int env, int n_envs, int key) {
+  const int s = persist_set(c, q.nch, par);
+  key = q.regroup ? key >> q.key_shift : 0;
+  const int b = key < 0 ? 0 : (key < LS_RANK_BUCKETS - 1 ? key : LS_RANK_BUCKETS - 1);
+  int* cnt = q.cnt + (size_t)s * 3 * LS_RANK_BUCKETS;
+  const int pos = atomicAdd(&cnt[b], 1);
+  st_relaxed(&q.benv[((size_t)s * LS_RANK_BUCKETS + b) * n_envs + pos], env);
+  __threadfence();
+  atomicAdd(&cnt[LS_RANK_BUCKETS + b], 1);
+  atomicAdd(&q.tot[2 * s], 1);
+}
+
+// next group (called by one whole warp): up to `want` envs of the lowest chunk whose ready envs reach the pool threshold
+// (pool x want, or all that remain of the chunk), hardest keys first; returns the number of envs (0: the step is done)
+__device__ __forceinline__ int persist_pop(const PersistQueue& q, int par, int n_envs, int want, int* s_env, int* chunk) {
+  const int lane = threadIdx.x & 31;
+  for (;;) {
+    if (ld_relaxed(&q.tot[2 * persist_set(q.nch - 1, q.nch, par) + 1]) >= n_envs) return 0;   // every env ran the last chunk
+    int c = -1, s = 0;
+    for (int k = 0; k < q.nch && c < 0; k++) {
+      s = persist_set(k, q.nch, par);
+      const int taken = ld_relaxed(&q.tot[2 * s + 1]);
+      if (taken >= n_envs) continue;
+      const int avail = ld_relaxed(&q.tot[2 * s]) - taken;
+      if (avail > 0 && avail >= min(q.pool * want, n_envs - taken)) c = k;
+    }
+    if (c < 0) { __nanosleep(256); continue; }
+    int* cnt = q.cnt + (size_t)s * 3 * LS_RANK_BUCKETS;
+    int* benv = q.benv + (size_t)s * LS_RANK_BUCKETS * n_envs;
+    int got = 0;
+    while (got < want) {
+      // lane l holds buckets 127 - 4 l .. 124 - 4 l: lane order is descending key order
+      int tk[4], a[4], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int b = LS_RANK_BUCKETS - 1 - 4 * lane - j;
+        tk[j] = ld_relaxed(&cnt[2 * LS_RANK_BUCKETS + b]);
+        a[j] = max(ld_relaxed(&cnt[LS_RANK_BUCKETS + b]) - tk[j], 0);
+        sum += a[j];
+      }
+      int incl = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+      if (__shfl_sync(0xffffffffu, incl, 31) == 0) break;
+      int above = incl - sum, mine = 0, g[4];
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int b = LS_RANK_BUCKETS - 1 - 4 * lane - j;
+        g[j] = min(max(want - got - above, 0), a[j]);
+        above += a[j];
+        if (g[j] > 0 && atomicCAS(&cnt[2 * LS_RANK_BUCKETS + b], tk[j], tk[j] + g[j]) != tk[j]) g[j] = 0;   // raced: retry
+        mine += g[j];
+      }
+      int off = mine;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, off, o); if (lane >= o) off += v; }
+      const int total = __shfl_sync(0xffffffffu, off, 31);
+      off += got - mine;
+      // the claimed slots, one per lane (a bucket often gives all of them): first their indices into s_env ...
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int b = LS_RANK_BUCKETS - 1 - 4 * lane - j;
+        for (int i = 0; i < g[j]; i++) s_env[off++] = b * n_envs + tk[j] + i;
+      }
+      __syncwarp();
+      if (lane < total) {
+        // ... then the env ids. A slot is reserved before its env id is stored: wait for the (running) publisher
+        int* slot = benv + s_env[got + lane];
+        int v;
+        while ((v = ld_relaxed(slot)) < 0) __nanosleep(32);
+        st_relaxed(slot, -1);
+        s_env[got + lane] = v;
+      }
+      __syncwarp();
+      if (lane == 0 && total > 0) atomicAdd(&q.tot[2 * s + 1], total);
+      got += total;
+    }
+    if (got > 0) {
+      __threadfence();            // (acquire: the envs' state is read after their ids)
+      *chunk = c;
+      return got;
+    }
+  }
+}
+
+// one chunk [k0, k1) of one env: substep_body with the env given, L1-bypassing loads, and the env published into the next
+// chunk's buckets; returns the warp's Newton iterations in the chunk
+template <class C>
+__device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, const DevTask& t, const SolverOpts& so,
+                                            const EngineState& st, const float* __restrict__ action,
+                                            float* __restrict__ obs, float* __restrict__ reward,
+                                            uint8_t* __restrict__ done, float* __restrict__ next_obs, int n_envs,
+                                            int auto_reset, uint64_t seed, int64_t env_off, int sync_substeps,
+                                            int key_mode_in, int stage_bytes, int env, bool ghost, int c,
+                                            const PersistQueue& q, int par) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int key_mode = key_mode_in & 0xffff;
+  const int k0 = c * q.chunk, k1 = min(k0 + q.chunk, t.n_substeps);
+  EnvS<C>& e = reinterpret_cast<EnvS<C>*>(smem_raw)[warp];
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv, nu = m.nu, D = t.obs_dim;
+  if (lane == 0) {
+    e.prm = st.pool + (size_t)__ldcg(&st.dr_row[env]) * m.pool_P;
+    if (stage_bytes > 0) {
+      const unsigned char* sm = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
+      e.pk_tab = reinterpret_cast<const int*>(sm);
+    } else { e.pk_tab = m.pair_packed; }
+  }
+
+  // ---- load state ----
+  for (int i = lane; i < nv; i += 32) {
+    e.qpos[i] = __ldcg(&st.qpos[(size_t)env * nv + i]);
+    e.qvel[i] = __ldcg(&st.qvel[(size_t)env * nv + i]);
+    e.qacc_ws[i] = __ldcg(&st.ws[(size_t)env * nv + i]);
+    e.qacc[i] = 0;
+  }
+  for (int i = lane; i < nu; i += 32) e.ctrl[t.act_idx[i]] = action[(size_t)env * nu + i] * t.act_delta[i] + t.act_mean[i];
+  if (lane < 4) e.goal[lane] = __ldcg(&st.goal[(size_t)env * 4 + lane]);
+  __syncwarp();
+  init_workspace(ms, e);
+  float rew = 0;
+  int* carry = q.carry + (size_t)env * LS_CARRY;
+  static_assert(EnvS<C>::NSEP <= 4 && 3 * LS_MAX_GRF <= 12, "carry record layout");
+  if (k0 > 0) {
+    // what the previous chunks of this control step left behind (init_workspace above cleared part of it)
+    if (lane == 0) {
+      e.iter_sum = __ldcg(&carry[0]); e.mpr_calls = __ldcg(&carry[1]); e.sep_next = __ldcg(&carry[2]);
+      rew = __int_as_float(__ldcg(&carry[3]));
+    }
+    if (lane < EnvS<C>::NSEP) e.sep_pair[lane] = __ldcg(&carry[4 + lane]);
+    if (lane < 3 * EnvS<C>::NSEP) (&e.sep_dir[0][0])[lane] = __int_as_float(__ldcg(&carry[8 + lane]));
+    if (lane < 3 * LS_MAX_GRF) e.grf[lane] = __int_as_float(__ldcg(&carry[20 + lane]));
+    __syncwarp();
+  } else {
+    if (lane == 0) e.iter_sum = 0;
+    if (lane < 3 * LS_MAX_GRF) e.grf[lane] = 0;
+    // reward depends on the *previous* observation only (utils/reward.py via base.py:170-176): evaluate it now
+    if (t.reward_type == LS_REWARD_TARGET_VELOCITY) { float d = obs_value(t, e, t.ri[0]) - t.rp[0]; rew = expf(-d * d); }
+    else if (t.reward_type == LS_REWARD_VELOCITY_VECTOR) {
+      float g = obs_value(t, e, t.ri[3]);
+      float dx = obs_value(t, e, t.ri[0]) - g * obs_value(t, e, t.ri[2]);
+      float dy = obs_value(t, e, t.ri[1]) - g * obs_value(t, e, t.ri[2] + 1);
+      rew = expf(-5.0f * sqrtf(dx * dx + dy * dy));
+    } else if (t.reward_type == LS_REWARD_POS) rew = obs_value(t, e, t.ri[0]);
+  }
+  const int iter0 = e.iter_sum, mpr0 = e.mpr_calls;    // (the regrouping key counts this chunk's sub-steps)
+
+  // ---- physics ----
+  if (sync_substeps) {
+    // keep the warps of a block in the same phase: they then share instruction-cache lines
+    for (int k = k0; k < k1; k++) { if (k % sync_substeps == 0) __syncthreads(); physics_substeps(ms, e, so, 1, t.grf_group, t.n_grf); }
+  } else {
+    physics_substeps(ms, e, so, k1 - k0, t.grf_group, t.n_grf);
+  }
+  const int iters = e.iter_sum - iter0;
+
+  if (k1 < t.n_substeps) {
+    // ---- not the last chunk of the control step: state and carried fields to HBM, env into the next chunk's bucket ----
+    if (!ghost) {
+      for (int i = lane; i < nv; i += 32) {
+        st.qpos[(size_t)env * nv + i] = e.qpos[i];
+        st.qvel[(size_t)env * nv + i] = e.qvel[i];
+        st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
+      }
+      if (lane == 0) { carry[0] = e.iter_sum; carry[1] = e.mpr_calls; carry[2] = e.sep_next; carry[3] = __float_as_int(rew); }
+      if (lane < EnvS<C>::NSEP) carry[4 + lane] = e.sep_pair[lane];
+      if (lane < 3 * EnvS<C>::NSEP) carry[8 + lane] = __float_as_int((&e.sep_dir[0][0])[lane]);
+      if (lane < 3 * LS_MAX_GRF) carry[20 + lane] = __float_as_int(e.grf[lane]);
+      __threadfence();
+      __syncwarp();
+      if (lane == 0) persist_publish(q, par, c + 1, env, n_envs, launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in));
+    }
+    return iters;
+  }
+  if (ghost) return iters;
+
+  // ---- observation, termination, reward ----
+  bool bad = false;
+  for (int i = lane; i < nv; i += 32) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+  bool fallen = false;
+  for (int k = lane; k < t.n_done; k += 32) {
+    float v = obs_value(t, e, t.done_obs_idx[k]);
+    fallen |= (v < t.done_lo[k]) || (v > t.done_hi[k]);
+  }
+  bad = __any_sync(0xffffffffu, bad);
+  fallen = __any_sync(0xffffffffu, fallen) && t.use_absorbing;
+  const bool is_done = fallen || bad;
+  if (t.reward_type == LS_REWARD_TRACKING) {
+    // mocap-tracking reward (include/locosim_task.h): the cursor advances one sample, the observation reached by this step
+    // is compared with the table row at the advanced cursor
+    int cur = st.cursor[env];
+    const int tj = cur / t.traj_len;
+    int sp = cur - tj * t.traj_len;
+    sp = sp + 1 < t.traj_len ? sp + 1 : t.traj_len - 1;
+    cur = tj * t.traj_len + sp;
+    const float* ref = t.table + (size_t)cur * (2 * nv + t.n_goal);
+    float ep = 0, ev = 0;
+    for (int k = lane; k < D; k += 32) {
+      const int ty = t.obs_src_type[k], idx = t.obs_src_idx[k];
+      if (ty == LS_OBS_QPOS) { const float d = e.qpos[idx] - ref[idx]; ep += d * d; }
+      else if (ty == LS_OBS_QVEL) { const float d = e.qvel[idx] - ref[nv + idx]; ev += d * d; }
+    }
+    ep = warp_sum(ep); ev = warp_sum(ev);
+    rew = bad ? 0.0f : t.track[0] * expf(-t.track[1] * ep) + t.track[2] * expf(-t.track[3] * ev);
+    if (lane == 0) st.cursor[env] = cur;
+  }
+  for (int k = lane; k < D; k += 32) {
+    float v = obs_value(t, e, k);
+    if (bad) v = 0.0f;
+    obs[(size_t)env * D + k] = v;
+  }
+  if (lane == 0) {
+    float r = rew;
+    reward[env] = r;
+    done[env] = is_done ? 1 : 0;
+    int* cnt = st.counters + (size_t)env * 8;
+    cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
+    if (bad) cnt[4] += 1;
+    {
+      int key = e.iter_sum;
+      const int mpr_w = (key_mode >> 8) & 255;           // weight of one MPR run in Newton-iteration units
+      key_mode &= 255;
+      if (key_mode == 1) key = (cnt[5] + e.iter_sum + 1) >> 1;
+      else if (key_mode == 2) key = e.solver_iter * 8;
+      else if (key_mode == 3) key = e.iter_sum + (e.nefc >> 1) + mpr_w * min(e.mpr_calls, 64);
+      else if (key_mode == 4) key = (3 * cnt[5] + e.iter_sum + 2) >> 2;
+      else if (key_mode == 5) key = e.iter_sum + 4 * e.solver_iter;
+      else if (key_mode == 6) key = e.iter_sum + e.nefc;
+      else if (key_mode == 7) key = e.iter_sum + 4 * e.solver_iter + (e.nefc >> 1);
+      cnt[5] = key;
+    } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
+  }
+
+  // ---- auto-reset ----
+  if (is_done && (auto_reset || bad)) {
+    const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
+    int ep = st.episode[env];
+    int tr, sp;
+    draw_reset(seed, env_off + env, ep, t.n_traj, t.traj_len, &tr, &sp);
+    __syncwarp();
+    reset_env(ms, t, e, tr, sp, t.rot[0] >= 0 ? draw_rot_angle(seed, env_off + env, ep) : 0.0f);
+    if (lane == 0) {
+      const int prow = draw_pool_row(seed, env_off + env, ep, st.pool_K);
+      st.episode[env] = ep + 1; st.counters[(size_t)env * 8 + 1] += 1;
+      if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
+      st.dr_row[env] = prow;
+      st.cursor[env] = tr * t.traj_len + sp;
+      e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
+    }
+    __syncwarp();
+    for (int k = lane; k < t.n_goal; k += 32) st.goal[(size_t)env * 4 + k] = e.goal[k];
+  }
+  if (next_obs) for (int k = lane; k < D; k += 32) next_obs[(size_t)env * D + k] = obs_value(t, e, k);
+
+  // ---- store state ----
+  for (int i = lane; i < nv; i += 32) {
+    st.qpos[(size_t)env * nv + i] = e.qpos[i];
+    st.qvel[(size_t)env * nv + i] = e.qvel[i];
+    st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
+  }
+  __threadfence();
+  __syncwarp();
+  if (lane == 0) {
+    // into chunk 0 of the next step
+    int key = launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in);
+    if (is_done && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
+    persist_publish(q, par, q.nch, env, n_envs, key);
+  }
+  return iters;
+}
+
+template <class C>
+__global__ void __launch_bounds__(512, 1) persist_kernel(int ms, DevTask t, SolverOpts so, EngineState st,
+                                                       const float* __restrict__ action, float* __restrict__ obs,
+                                                       float* __restrict__ reward, uint8_t* __restrict__ done,
+                                                       float* __restrict__ next_obs, int n_envs, int auto_reset,
+                                                       uint64_t seed, int64_t env_off, int sync_substeps, int key_mode_in,
+                                                       const unsigned char* __restrict__ stage_src, int stage_bytes,
+                                                       PersistQueue q) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ int s_env[16], s_n, s_c, s_par, s_it[2];
+  __shared__ long long s_t[2];   // timeline: pop start, group start (in shared memory: nothing extra live across the body)
+  const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+  if (stage_bytes > 0) {
+    // the TMA-staged pair table of step_kernel, once per block for the whole step
+    unsigned char* dst = smem_raw + (size_t)wpb * sizeof(EnvS<C>);
+    const unsigned dst_a = (unsigned)__cvta_generic_to_shared(dst);
+    const unsigned bar_a = dst_a + (unsigned)stage_bytes;
+    if (threadIdx.x == 0) {
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"((unsigned)stage_bytes) : "memory");
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
+                   "l"(stage_src), "r"((unsigned)stage_bytes), "r"(bar_a)
+                   : "memory");
+    }
+    __syncthreads();                                    // (the barrier object is initialised before anybody polls it)
+    unsigned ok = 0;
+    while (!ok)
+      asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                   : "=r"(ok) : "r"(bar_a) : "memory");
+  }
+  if (threadIdx.x == 0) s_par = __ldcg(&q.seq[0]) & 1;
+  __syncthreads();
+  for (;;) {
+    if (q.tl && threadIdx.x == 0) { s_t[0] = global_ns(); s_it[0] = 0; s_it[1] = 0; }
+    if (warp == 0) {
+      int c = 0;
+      const int n = persist_pop(q, s_par, n_envs, wpb, s_env, &c);
+      if (threadIdx.x == 0) { s_n = n; s_c = c; }
+    }
+    __syncthreads();
+    const int n = s_n;
+    if (n == 0) break;
+    if (q.tl && threadIdx.x == 0) s_t[1] = global_ns();
+    // warps past the group's last env shadow it (same barriers, no stores)
+    const bool ghost = warp >= n;
+    const int it = persist_body<C>(smem_raw, ms, t, so, st, action, obs, reward, done, next_obs, n_envs, auto_reset, seed,
+                                   env_off, sync_substeps, key_mode_in, stage_bytes, s_env[ghost ? n - 1 : warp], ghost, s_c,
+                                   q, s_par);
+    if (q.tl && (threadIdx.x & 31) == 0) { if (!ghost) atomicAdd(&s_it[0], it); atomicMax(&s_it[1], it); }
+    __syncthreads();
+    if (q.tl && threadIdx.x == 0) {
+      const long long r = (long long)atomicAdd((unsigned long long*)q.tl, 1ULL);
+      if (r < q.tl_cap) {
+        unsigned smid;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+        long long* rec = q.tl + (r + 1) * LS_TL_WORDS;
+        rec[0] = smid; rec[1] = s_c; rec[2] = n; rec[3] = s_t[0]; rec[4] = s_t[1]; rec[5] = global_ns(); rec[6] = s_it[0]; rec[7] = s_it[1];
+      }
+    }
+  }
+  // The block that finishes last (every env has run every chunk by then) empties the bucket sets of this step's chunks; the
+  // set the last chunk filled becomes chunk 0 of the next step. No host-side counter, so CUDA graphs replay it.
+  int last = 0;
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last = atomicAdd(&q.seq[1], 1) == (int)gridDim.x - 1;
+  }
+  if (__syncthreads_or(last)) {
+    __threadfence();
+    const int par = s_par;
+    for (int c = 0; c < q.nch; c++) {
+      const int s = persist_set(c, q.nch, par);
+      for (int i = threadIdx.x; i < 3 * LS_RANK_BUCKETS; i += blockDim.x) q.cnt[(size_t)s * 3 * LS_RANK_BUCKETS + i] = 0;
+      if (threadIdx.x < 2) q.tot[2 * s + threadIdx.x] = 0;
+    }
+    if (threadIdx.x == 0) { q.seq[0] = par ^ 1; q.seq[1] = 0; }
+  }
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // Regrouping: the warps of a block run the solver in lock-step, so a block is as slow as its hardest env. Solver effort
 // is strongly correlated from one control step to the next (lag-1 correlation of the per-step Newton iteration count
 // ~0.6), so before every step the envs are bucketed by the iteration count of their previous step (counting sort,
@@ -606,6 +1004,9 @@ struct locosim_handle {
   int n_sm = 1;
   int resort = 0;                   // sub-steps per launch of the step kernel (>= n_substeps: one fused launch per step)
   SplitState split = {};
+  int persist = 0, persist_grid = 0;   // resort < n_substeps: one persist_kernel launch of persist_grid blocks per step
+  int persist_static = 0;              // static shared memory of persist_kernel<C> (bytes)
+  PersistQueue pq = {};
   uint64_t seed = 0;
   int64_t env_off = 0;
   HostModel hm;
@@ -651,6 +1052,10 @@ static int launch_step(locosim_handle* h, const float* a, float* o, float* r, ui
     step_kernel<C><<<blocks, h->wpb * 32, smem, s>>>(h->slot, h->dt, h->so, h->st, a, o, r, d, no, h->n_envs, auto_reset,
                                                       h->seed, h->env_off, h->sync_substeps, h->key_mode, h->d_stage,
                                                       h->stage_bytes);
+  } else if (h->persist) {
+    persist_kernel<C><<<h->persist_grid, h->wpb * 32, smem, s>>>(h->slot, h->dt, h->so, h->st, a, o, r, d, no, h->n_envs,
+                                                                 auto_reset, h->seed, h->env_off, h->sync_substeps,
+                                                                 h->key_mode, h->d_stage, h->stage_bytes, h->pq);
   } else {
     for (int k0 = 0; k0 < nsub; k0 += h->resort)
       substep_kernel<C><<<blocks, h->wpb * 32, smem, s>>>(h->slot, h->dt, h->so, h->st, a, o, r, d, no, h->n_envs, auto_reset,
@@ -719,9 +1124,51 @@ static int setup_cfg(locosim_handle* h) {
     const int nsub = h->dt.n_substeps;
     const bool full = (h->n_envs + best - 1) / best >= h->n_sm;
     h->resort = full && C::CONE == 1 && !C::RK4 ? 2 : nsub;
+    // ... and all of them in one persistent launch (persist_kernel) where the sub-step split is the default; LOCOSIM_RESORT
+    // alone selects the separate launches, LOCOSIM_PERSIST=1 the persistent kernel with LOCOSIM_RESORT sub-steps per chunk
+    h->persist = h->resort < nsub && !getenv("LOCOSIM_RESORT");
     if (getenv("LOCOSIM_RESORT")) h->resort = atoi(getenv("LOCOSIM_RESORT"));
     if (h->resort < 1 || h->resort > nsub) h->resort = nsub;
-    if (h->resort < nsub) {
+    if (getenv("LOCOSIM_PERSIST")) h->persist = atoi(getenv("LOCOSIM_PERSIST")) > 0;
+    if (h->resort >= nsub) h->persist = 0;
+    if (h->persist) {
+      // bucket sets: chunk 0 of this step and of the next alternate between sets 0 and 1, chunks 1 .. nch-1 use 2 .. nch
+      const size_t N = (size_t)h->n_envs;
+      PersistQueue& q = h->pq;
+      q.chunk = h->resort;
+      q.nch = (nsub + h->resort - 1) / h->resort;
+      const size_t sets = (size_t)q.nch + 1;
+      q.pool = 2;                  // ready envs before a block takes a group of a chunk: pool x wpb (or all the chunk has left)
+      if (getenv("LOCOSIM_PERSIST_POOL")) q.pool = atoi(getenv("LOCOSIM_PERSIST_POOL"));
+      if (q.pool < 0) q.pool = 0;
+      q.regroup = h->regroup;
+      q.key_shift = h->key_shift;
+      CK(cudaMalloc((void**)&q.carry, N * LS_CARRY * 4));
+      CK(cudaMalloc((void**)&q.cnt, sets * 3 * LS_RANK_BUCKETS * 4));
+      CK(cudaMalloc((void**)&q.tot, sets * 2 * 4));
+      CK(cudaMalloc((void**)&q.benv, sets * LS_RANK_BUCKETS * N * 4));
+      CK(cudaMalloc((void**)&q.seq, 2 * 4));
+      CK(cudaMemset(q.carry, 0, N * LS_CARRY * 4));
+      CK(cudaMemset(q.cnt, 0, sets * 3 * LS_RANK_BUCKETS * 4));
+      CK(cudaMemset(q.tot, 0, sets * 2 * 4));
+      CK(cudaMemset(q.benv, 0xff, sets * LS_RANK_BUCKETS * N * 4));
+      CK(cudaMemset(q.seq, 0, 2 * 4));
+      // the first step reads set 0: every env published in bucket 0, in env order
+      const int n = h->n_envs, cnt0[2] = {n, n};
+      CK(cudaMemcpy(q.cnt, &cnt0[0], 4, cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(q.cnt + LS_RANK_BUCKETS, &cnt0[1], 4, cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(q.tot, &n, 4, cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(q.benv, h->st.perm, N * 4, cudaMemcpyDeviceToDevice));
+      // one resident block per SM; LOCOSIM_PERSIST_GRID caps the grid (any number of blocks makes progress)
+      const int blocks = (h->n_envs + best - 1) / best;
+      h->persist_grid = blocks < h->n_sm ? blocks : h->n_sm;
+      if (getenv("LOCOSIM_PERSIST_GRID")) { int g = atoi(getenv("LOCOSIM_PERSIST_GRID")); if (g >= 1 && g < h->persist_grid) h->persist_grid = g; }
+      // (its few static shared variables come out of the same 227 KB: the TMA staging below leaves room for them)
+      cudaFuncAttributes fa;
+      CK(cudaFuncGetAttributes(&fa, persist_kernel<C>));
+      h->persist_static = (int)fa.sharedSizeBytes;
+      CK(cudaFuncSetAttribute(persist_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, dev_max - h->persist_static));
+    } else if (h->resort < nsub) {
       const size_t N = (size_t)h->n_envs;
       CK(cudaMalloc((void**)&h->split.carry, N * LS_CARRY * 4));
       CK(cudaMalloc((void**)&h->split.bcount, 2 * LS_RANK_BUCKETS * 4));
@@ -756,7 +1203,7 @@ static int setup_cfg(locosim_handle* h) {
     // the PRIMITIVE part of the table (the lean loop over the convex part streams the model's table from L2)
     const int np = h->hm.np_prim;
     const int bytes = (2 * np * 4 + 15) & ~15;                   // np packed pairs directly followed by np bounds
-    if (np > 0 && h->smem + bytes + 16 <= dev_max) {
+    if (np > 0 && h->smem + bytes + 16 <= dev_max - h->persist_static) {
       CK(cudaMalloc((void**)&h->d_stage, bytes));
       CK(cudaMemset(h->d_stage, 0, bytes));
       CK(cudaMemcpy(h->d_stage, h->dm.pair_packed, 4 * np, cudaMemcpyDeviceToDevice));
@@ -850,6 +1297,7 @@ void locosim_destroy(locosim_t* h) {
   cudaFree(h->st.counters); cudaFree(h->st.dr_row); cudaFree(h->st.perm); cudaFree(h->st.cursor); cudaFree(h->d_pool);
   cudaFree(h->d_stage);
   cudaFree(h->split.carry); cudaFree(h->split.bcount); cudaFree(h->split.benv); cudaFree(h->split.seq);
+  cudaFree(h->pq.carry); cudaFree(h->pq.cnt); cudaFree(h->pq.tot); cudaFree(h->pq.benv); cudaFree(h->pq.seq);
   delete h;
 }
 
@@ -996,8 +1444,15 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
 
 int locosim_kernels_per_step(const locosim_t* h) {
   const int nsub = h->dt.n_substeps;
+  if (h->persist) return 1;
   if (h->resort < nsub) return (nsub + h->resort - 1) / h->resort;
   return h->regroup ? 2 : 1;
+}
+int locosim_set_timeline(locosim_t* h, long long* d_records, int capacity) {
+  if (!h->persist) { h->err = "the timeline is recorded by the persistent sub-step kernel only"; return 1; }
+  h->pq.tl = capacity > 0 ? d_records : nullptr;
+  h->pq.tl_cap = capacity;
+  return 0;
 }
 int locosim_debug_counters(unsigned long long* out8) {
   return cudaMemcpyFromSymbol(out8, g_dbg, 64) == cudaSuccess ? 0 : 1;

@@ -72,6 +72,8 @@ def load_library():
     lib.locosim_measure_fp32_peak.argtypes = [ip, ctypes.POINTER(ctypes.c_double)]
     lib.locosim_launch_info.restype = ip
     lib.locosim_launch_info.argtypes = [vp, ctypes.POINTER(ip), ctypes.POINTER(ip), ctypes.POINTER(ip)]
+    lib.locosim_set_timeline.restype = ip
+    lib.locosim_set_timeline.argtypes = [vp, vp, ip]
     _LIB = lib
     return lib
 
@@ -82,7 +84,7 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_param_pool_row_len", "locosim_set_param_pool", "locosim_get_param_rows",
                     "locosim_kernels_per_step", "locosim_reset_rows", "locosim_set_goal", "locosim_measure_fp32_peak",
                     "locosim_set_reset_rotation", "locosim_get_cursor", "locosim_dataset_rows", "locosim_create_dataset",
-                    "locosim_debug_counters"]
+                    "locosim_debug_counters", "locosim_set_timeline"]
 
 
 def measure_fp32_peak(device=0):
