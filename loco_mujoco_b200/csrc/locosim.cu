@@ -59,6 +59,7 @@ __device__ __forceinline__ int draw_pool_row(uint64_t seed, int64_t genv, int ep
   return (int)(r % (uint64_t)K);
 }
 
+#ifndef LOCOSIM_EXTRA_CONFIGS_TU   // (locosim_configs31.cu: the second translation unit compiles the step kernels only)
 // ----------------------------------------------------------------------------------------------------------
 // reset kernel: one warp per env, no shared memory
 // ----------------------------------------------------------------------------------------------------------
@@ -104,6 +105,7 @@ __global__ void reset_kernel(int ms, DevTask t, EngineState st, const uint8_t* m
     st.cursor[env] = tr * t.traj_len + sp;
   }
 }
+#endif
 
 // ----------------------------------------------------------------------------------------------------------
 // Sub-step launches (LOCOSIM_RESORT = S < n_substeps): the control step runs as ceil(n_substeps / S) launches of the step
@@ -1020,8 +1022,10 @@ struct locosim_handle {
   unsigned char* d_stage = nullptr; int stage_bytes = 0;
   std::string err;
 };
+#ifndef LOCOSIM_EXTRA_CONFIGS_TU
 static std::string g_create_error;
 static bool g_slot_used[LS_MAX_SLOTS] = {false};
+#endif
 
 #define CK(call)                                                                      \
   do {                                                                                \
@@ -1218,6 +1222,15 @@ static int setup_cfg(locosim_handle* h) {
   return 0;
 }
 
+#ifndef LOCOSIM_EXTRA_CONFIGS_TU
+// The 31-dof configurations (CfgPyrRK4_31, CfgPyrEuler31) are compiled in their own translation unit,
+// locosim_configs31.cu, linked into the same library (two nvcc processes build the library in parallel). Their entry points
+// are weak: a library built from this file alone reports those models as not compiled in.
+extern "C" int locosim_configs31_setup(locosim_handle* h) __attribute__((weak));
+extern "C" int locosim_configs31_step(locosim_handle* h, const float* a, float* o, float* r, uint8_t* d, float* no,
+                                      int auto_reset, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_configs31_sync_model(locosim_handle* h) __attribute__((weak));
+
 extern "C" {
 
 const char* locosim_last_error(const locosim_t* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
@@ -1282,6 +1295,15 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
     case 0: rc = setup_cfg<CfgEllEuler>(h); break;
     case 1: rc = setup_cfg<CfgPyrEuler>(h); break;
     case 3: rc = setup_cfg<CfgPyrEuler29>(h); break;
+    case 4:
+    case 5:
+      if (!locosim_configs31_setup) { h->err = "the 31-dof configurations are not compiled into this library"; rc = 1; break; }
+      rc = locosim_configs31_setup(h);
+      // (this unit's reset / dataset kernels read the model from its own __constant__ slots: same descriptor, staging included)
+      if (!rc && cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess) {
+        h->err = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); rc = 1;
+      }
+      break;
     default: rc = setup_cfg<CfgPyrRK4>(h); break;
   }
   if (rc) { g_create_error = h->err; locosim_destroy(h); return 1; }
@@ -1371,6 +1393,8 @@ int locosim_step(locosim_t* h, const float* a, float* o, float* r, uint8_t* d, f
     case 0: return launch_step<CfgEllEuler>(h, a, o, r, d, no, auto_reset, s);
     case 1: return launch_step<CfgPyrEuler>(h, a, o, r, d, no, auto_reset, s);
     case 3: return launch_step<CfgPyrEuler29>(h, a, o, r, d, no, auto_reset, s);
+    case 4:
+    case 5: return locosim_configs31_step(h, a, o, r, d, no, auto_reset, s);
     default: return launch_step<CfgPyrRK4>(h, a, o, r, d, no, auto_reset, s);
   }
 }
@@ -1438,6 +1462,7 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
   h->dm.nfric = nfric;
   if (damp) h->dm.has_damping = 1;
   CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   CK(cudaMemset(h->st.dr_row, 0, (size_t)h->n_envs * 4));
   return 0;
 }
@@ -1511,3 +1536,4 @@ int locosim_launch_info(const locosim_t* h, int* wpb, int* smem, int* blocks) {
 }
 
 }  // extern "C"
+#endif  // LOCOSIM_EXTRA_CONFIGS_TU

@@ -1,0 +1,65 @@
+// locosim_configs31.cu -- the step kernels of the two 31-dof configurations (locosim_config.h: CfgPyrRK4_31 for Atlas with
+// arms, CfgPyrEuler31 for Talos with arms), in a translation unit of their own that is linked into the engine library
+// next to locosim.cu. It compiles the kernel templates of locosim.cu (step, sub-step and persistent kernels, launch and
+// setup) for these two configurations only; the handle, the C-ABI and the reset / dataset / regrouping kernels stay in
+// locosim.cu, which calls the entry points below for configuration indices 4 and 5.
+//
+// Each translation unit has its own __constant__ model slots (no relocatable device code): this unit's slot of a handle is
+// written here at setup and after a parameter-pool upload, locosim.cu writes its own. The engine source is compiled inside
+// namespace locosim31 so that its external device functions (the __noinline__ phases) do not collide with locosim.cu's at
+// link time; the system and ABI headers are included first, outside it.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/locosim.h"
+#include "../../include/locosim_modelpack.h"
+#include "../../include/locosim_task.h"
+
+#define LOCOSIM_EXTRA_CONFIGS_TU 1
+namespace locosim31 {
+#include "locosim.cu"
+
+// sizeof(EnvS) decides the envs resident per SM (see locosim.cu)
+static_assert(sizeof(EnvS<CfgPyrRK4_31>) * 8 <= 232448, "Atlas with arms: 8 envs per SM");
+static_assert(sizeof(EnvS<CfgPyrEuler31>) * 8 <= 232448, "Talos with arms: 8 envs per SM");
+}  // namespace locosim31
+
+// the handle is locosim.cu's (the same struct definition, compiled in both units)
+typedef locosim31::locosim_handle Handle31;
+
+extern "C" {
+
+int locosim_configs31_sync_model(Handle31* h) {
+  using namespace locosim31;
+  CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
+  return 0;
+}
+
+int locosim_configs31_setup(Handle31* h) {
+  using namespace locosim31;
+  if (locosim_configs31_sync_model(h)) return 1;
+  switch (h->cfg) {
+    case 4: return setup_cfg<CfgPyrRK4_31>(h);
+    case 5: return setup_cfg<CfgPyrEuler31>(h);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
+int locosim_configs31_step(Handle31* h, const float* a, float* o, float* r, uint8_t* d, float* no, int auto_reset,
+                           cudaStream_t s) {
+  using namespace locosim31;
+  switch (h->cfg) {
+    case 4: return launch_step<CfgPyrRK4_31>(h, a, o, r, d, no, auto_reset, s);
+    case 5: return launch_step<CfgPyrEuler31>(h, a, o, r, d, no, auto_reset, s);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
+}

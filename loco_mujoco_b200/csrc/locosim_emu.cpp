@@ -103,6 +103,8 @@ EmuBase* emu_create(const int* ints, int n_ints, const double* reals, int n_real
     case 1: s = new EmuT<CfgPyrEuler>(); break;
     case 2: s = new EmuT<CfgPyrRK4>(); break;
     case 3: s = new EmuT<CfgPyrEuler29>(); break;
+    case 4: s = new EmuT<CfgPyrRK4_31>(); break;
+    case 5: s = new EmuT<CfgPyrEuler31>(); break;
     default: fprintf(stderr, "emu: no compiled configuration fits this model\n"); return nullptr;
   }
   s->hm = hm;
@@ -138,6 +140,8 @@ int emu_sizeof_env(int which) {
     case 0: return (int)sizeof(EnvS<CfgEllEuler>);
     case 1: return (int)sizeof(EnvS<CfgPyrEuler>);
     case 3: return (int)sizeof(EnvS<CfgPyrEuler29>);
+    case 4: return (int)sizeof(EnvS<CfgPyrRK4_31>);
+    case 5: return (int)sizeof(EnvS<CfgPyrEuler31>);
     default: return (int)sizeof(EnvS<CfgPyrRK4>);
   }
 }

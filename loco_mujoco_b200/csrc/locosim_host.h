@@ -192,12 +192,15 @@ static inline bool cfg_fits(const HostModel& hm, int obs_dim) {
   return hm.nv <= C::NV && hm.nb <= C::NB && hm.ng <= C::NG && obs_dim <= C::MAXOBS && hm.cone == (int)C::CONE &&
          hm.integrator == (int)C::RK4;
 }
-// 0 CfgEllEuler, 1 CfgPyrEuler, 2 CfgPyrRK4, 3 CfgPyrEuler29, -1 none fits (the first that fits wins)
+// 0 CfgEllEuler, 1 CfgPyrEuler, 2 CfgPyrRK4, 3 CfgPyrEuler29, 4 CfgPyrRK4_31, 5 CfgPyrEuler31, -1 none fits (the first
+// that fits wins, so a model keeps the smallest configuration it fits)
 static inline int select_cfg(const HostModel& hm, int obs_dim) {
   if (cfg_fits<CfgEllEuler>(hm, obs_dim)) return 0;
   if (cfg_fits<CfgPyrEuler>(hm, obs_dim)) return 1;
   if (cfg_fits<CfgPyrRK4>(hm, obs_dim)) return 2;
   if (cfg_fits<CfgPyrEuler29>(hm, obs_dim)) return 3;
+  if (cfg_fits<CfgPyrRK4_31>(hm, obs_dim)) return 4;
+  if (cfg_fits<CfgPyrEuler31>(hm, obs_dim)) return 5;
   return -1;
 }
 

@@ -126,6 +126,18 @@ def reference_data_root():
 ASSET_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "assets")
 
 
+def asset_path(rel):
+    """Path of a compiled asset (`<task>.npz`, `dr_pools/<task>.npz`): the package's own ASSET_DIR first, then the
+    directories listed in LOCO_MUJOCO_B200_ASSET_PATH (os.pathsep-separated; e.g. the full-body variants shipped as test
+    fixtures under tests/golden/full_body). None if no directory has it."""
+    extra = [d for d in os.environ.get("LOCO_MUJOCO_B200_ASSET_PATH", "").split(os.pathsep) if d]
+    for d in [ASSET_DIR] + extra:
+        path = os.path.join(d, rel)
+        if os.path.exists(path):
+            return path
+    return None
+
+
 class LocoEnv:
     """Base class of all batched locomotion environments."""
 
@@ -354,8 +366,8 @@ class LocoEnv:
         made; for the reference's shipped YAML configs a pre-built seeded pool is bundled (tools/build_dr_pools.py)."""
         import json
         task_id = getattr(self, "_task_id", None)
-        path = os.path.join(ASSET_DIR, "dr_pools", "%s.npz" % task_id)
-        if task_id is None or not os.path.exists(path):
+        path = asset_path(os.path.join("dr_pools", "%s.npz" % task_id)) if task_id is not None else None
+        if path is None:
             raise ValueError("domain randomisation needs the MJCF source (a loco_mujoco checkout); no pre-built pool is "
                              "bundled for %s" % task_id)
         d = np.load(path, allow_pickle=False)

@@ -4,6 +4,7 @@ Mirrors /root/reference/loco_mujoco/environments/humanoids/base_robot_humanoid.p
 atlas.py:275-453,485-598, talos.py:266-466,523-640 and unitreeH1.py:235-296,319-384,447-553 (joint/motor removal,
 observation/action specification, _has_fallen windows).
 """
+import inspect
 import os
 import warnings
 
@@ -11,7 +12,7 @@ import numpy as np
 
 from .. import mjcf
 from ..utils.checks import check_validity_task_mode_dataset
-from .base import LocoEnv, ObservationType, ValidTaskConf, reference_data_root, ASSET_DIR
+from .base import LocoEnv, ObservationType, ValidTaskConf, reference_data_root, asset_path
 
 _PELVIS = ["pelvis_tx", "pelvis_tz", "pelvis_ty", "pelvis_tilt", "pelvis_list", "pelvis_rotation"]
 _ARMS = ["%s_arm_%s" % (s, j) for s in ("l", "r") for j in ("shz", "shx", "ely", "elx", "wry", "wrx")]
@@ -91,7 +92,11 @@ class BaseRobotHumanoid(LocoEnv):
         if task not in ("walk", "run", "carry"):
             raise NotImplementedError("task %r is not built yet" % task)
         if task == "carry":
+            # base_robot_humanoid.py: the carried weight needs the arms fixed (asserted before any asset is looked up)
+            assert kwargs.get("disable_arms", True) is True, "If you want the robot to carry a weight, please disable " \
+                                                             "the arms. They will be kept fixed."
             kwargs["hold_weight"] = True
+        variant = cls.variant_suffix(**kwargs)
         reward_type = kwargs.pop("reward_type", "target_velocity")
         reward_params = kwargs.pop("reward_params", dict(target_velocity=2.5 if task == "run" else 1.25))
         root = reference_data_root()
@@ -107,7 +112,15 @@ class BaseRobotHumanoid(LocoEnv):
                                      clip_trajectory_to_joint_ranges=clip_trajectory_to_joint_ranges), warn=False)
         else:
             from .. import modelpack
-            asset = np.load(os.path.join(ASSET_DIR, "%s.%s.npz" % (cls.__name__, task)), allow_pickle=False)
+            path = asset_path("%s.%s%s.npz" % (cls.__name__, task, variant))
+            if path is None:
+                raise FileNotFoundError(
+                    "no bundled asset for %s.%s%s (%s): the package bundles the default models; other variants are "
+                    "compiled from a loco_mujoco checkout (set LOCO_MUJOCO_PATH) or read from a directory of assets made "
+                    "by tools/build_assets.py (set LOCO_MUJOCO_B200_ASSET_PATH)"
+                    % (cls.__name__, task, variant,
+                       ", ".join("%s=%s" % kv for kv in sorted(cls._variant_kwargs(kwargs).items()))))
+            asset = np.load(path, allow_pickle=False)
             n_models = int(asset["n_models"]) if "n_models" in asset.files else 1
             if n_models > 1:
                 model = [modelpack.from_npz_dict({k[len("model%d_" % i):]: asset[k] for k in asset.files
@@ -116,8 +129,26 @@ class BaseRobotHumanoid(LocoEnv):
                 model = modelpack.from_npz_dict({k[6:]: asset[k] for k in asset.files if k.startswith("model_")})
             mdp = cls(reward_type=reward_type, reward_params=reward_params, compiled_model=model, **kwargs)
             mdp.load_trajectory(dict(processed={k[5:]: asset[k] for k in asset.files if k.startswith("traj_")}))
-        mdp._task_id = "%s.%s" % (cls.__name__, task)
+        mdp._task_id = "%s.%s%s" % (cls.__name__, task, variant)
         return mdp
+
+    @classmethod
+    def _variant_kwargs(cls, kwargs):
+        """The model-variant options of a constructor call, with the class's defaults filled in."""
+        params = inspect.signature(cls.__init__).parameters
+        return {k: kwargs.get(k, params[k].default) for k in ("disable_arms", "disable_back_joint")}
+
+    @classmethod
+    def variant_suffix(cls, **kwargs):
+        """Suffix that names a model variant in asset and DR-pool file names: "" for the class's default model, else
+        "+arms" / "+back" for a part enabled that the default disables ("-arms" / "-back" for the reverse), e.g.
+        Atlas(disable_arms=False, disable_back_joint=False) -> "+arms+back"."""
+        params, chosen = inspect.signature(cls.__init__).parameters, cls._variant_kwargs(kwargs)
+        suffix = ""
+        for key, part in (("disable_arms", "arms"), ("disable_back_joint", "back")):
+            if chosen[key] != params[key].default:
+                suffix += ("-" if chosen[key] else "+") + part
+        return suffix
 
 
 class Atlas(BaseRobotHumanoid):

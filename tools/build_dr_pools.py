@@ -27,11 +27,15 @@ from loco_mujoco_b200.environments.base import ASSET_DIR              # noqa: E4
 
 REF = os.environ.get("LOCO_MUJOCO_PATH", "/root/reference/loco_mujoco")
 K, SEED = 64, 0
-JOBS = [("Atlas.walk", "atlas/domain_randomization_atlas.yaml", []),
-        ("Talos.walk", "talos/domain_randomization_talos.yaml", [("Inertial", "leg_right_5_link", "fullinertia")])]
+TALOS_DROP = [("Inertial", "leg_right_5_link", "fullinertia")]
+# (pool name = task + model variant, shipped YAML, dropped entries, model-variant kwargs)
+JOBS = [("Atlas.walk", "atlas/domain_randomization_atlas.yaml", [], {}),
+        ("Talos.walk", "talos/domain_randomization_talos.yaml", TALOS_DROP, {}),
+        ("Atlas.walk+arms", "atlas/domain_randomization_atlas.yaml", [], dict(disable_arms=False)),
+        ("Talos.walk+arms", "talos/domain_randomization_talos.yaml", TALOS_DROP, dict(disable_arms=False))]
 
-os.makedirs(os.path.join(ASSET_DIR, "dr_pools"), exist_ok=True)
-for task, rel, drop in JOBS:
+VARIANT_DIR = os.path.join(ROOT, "tests", "golden", "full_body")       # pools of model variants: data fixtures
+for task, rel, drop, variant in JOBS:
     conf = yaml.safe_load(open(os.path.join(REF, "environments", "data", rel)))
     shipped = copy.deepcopy(conf)
     for sec, name, key in drop:
@@ -39,11 +43,14 @@ for task, rel, drop in JOBS:
         if not conf[sec][name]:
             del conf[sec][name]
     np.random.seed(SEED)
-    env = LocoEnv.make(task + ".real", debug=True, domain_randomization_config=conf, domain_randomization_pool_size=K)
+    env = LocoEnv.make(task.split("+")[0] + ".real", debug=True, domain_randomization_config=conf,
+                       domain_randomization_pool_size=K, **variant)
+    assert env._task_id == task, (env._task_id, task)
     pool = env.domain_randomization_pool()
     meta = dict(task=task, yaml=os.path.basename(rel), seed=SEED, rows=K, dropped=[list(d) for d in drop],
                 config_used=conf, config_shipped=shipped)
-    out = os.path.join(ASSET_DIR, "dr_pools", task + ".npz")
+    out = os.path.join(VARIANT_DIR if variant else ASSET_DIR, "dr_pools", task + ".npz")
+    os.makedirs(os.path.dirname(out), exist_ok=True)
     np.savez_compressed(out, pool=pool, meta=np.array(json.dumps(meta)))
     spread = np.abs(pool - pool[0]).max(axis=0)
     print(task, pool.shape, "columns that vary:", int((spread > 0).sum()), "->", out, os.path.getsize(out), "bytes")
