@@ -713,6 +713,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
                                             int auto_reset, uint64_t seed, int64_t env_off, int sync_substeps,
                                             int key_mode_in, int stage_bytes, int env, bool ghost, int c,
                                             const PersistQueue& q, int par) {
+  PH_T0(t_ph);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int key_mode = key_mode_in & 0xffff;
   const int k0 = c * q.chunk, k1 = min(k0 + q.chunk, t.n_substeps);
@@ -764,6 +765,8 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
     } else if (t.reward_type == LS_REWARD_POS) rew = obs_value(t, e, t.ri[0]);
   }
   const int iter0 = e.iter_sum, mpr0 = e.mpr_calls;    // (the regrouping key counts this chunk's sub-steps)
+  PH_LAP(PH_PROLOGUE, t_ph);
+  PH_CNT(PH_GROUPS, 1);
 
   // ---- physics ----
   if (sync_substeps) {
@@ -773,6 +776,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
     physics_substeps(ms, e, so, k1 - k0, t.grf_group, t.n_grf);
   }
   const int iters = e.iter_sum - iter0;
+  PH_T0(t_epi);
 
   if (k1 < t.n_substeps) {
     // ---- not the last chunk of the control step: state and carried fields to HBM, env into the next chunk's bucket ----
@@ -790,6 +794,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
       __syncwarp();
       if (lane == 0) persist_publish(q, par, c + 1, env, n_envs, launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in));
     }
+    PH_LAP(PH_EPILOGUE, t_epi);
     return iters;
   }
   if (ghost) return iters;
@@ -886,6 +891,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
     if (is_done && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
     persist_publish(q, par, q.nch, env, n_envs, key);
   }
+  PH_LAP(PH_EPILOGUE, t_epi);
   return iters;
 }
 
@@ -1482,6 +1488,19 @@ int locosim_set_timeline(locosim_t* h, long long* d_records, int capacity) {
 int locosim_debug_counters(unsigned long long* out8) {
   return cudaMemcpyFromSymbol(out8, g_dbg, 64) == cudaSuccess ? 0 : 1;
 }
+#ifdef LOCOSIM_PHASE_CLOCK
+// (diagnostic build only) the phase clock summed over all slots into out[PH_N], then cleared; returns PH_N, or -1
+int locosim_phase_clock(unsigned long long* out) {
+  static unsigned long long buf[LS_PH_SLOTS][PH_N];
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(buf, g_phase, sizeof(buf)) != cudaSuccess) return -1;
+  for (int p = 0; p < PH_N; p++) {
+    out[p] = 0;
+    for (int s = 0; s < LS_PH_SLOTS; s++) out[p] += buf[s][p];
+  }
+  memset(buf, 0, sizeof(buf));
+  return cudaMemcpyToSymbol(g_phase, buf, sizeof(buf)) == cudaSuccess ? PH_N : -1;
+}
+#endif
 
 // Measured non-tensor FP32 peak (the denominator of the FP32 utilisation bench.py reports next to the HBM roofline):
 // 8 independent FMA chains per thread, 2 x 256 threads per SM slot, all SMs, best of 5 launches.

@@ -139,6 +139,30 @@ __constant__ int c_debug;      // diagnostic switches (LOCOSIM_DEBUG): 1 skip MP
 __device__ unsigned long long g_dbg[8];      // (LOCOSIM_DEBUG & 8) MPR statistics: calls, support pairs, hits, cap exits
 #endif
 
+// Phase clock: a diagnostic build (-DLOCOSIM_PHASE_CLOCK, tools/phase_profile.py) in which lane 0 of every warp adds the
+// clock64() cycles its env spends in each phase (or a count) to g_phase[slot][phase], one slot per (block mod 256, warp).
+// Without the macro the hooks expand to nothing, so the product library's code is the same as without them.
+enum {
+  PH_KINEMATICS, PH_COM_POS, PH_CRB_FACTOR, PH_SMOOTH_FORCES, PH_COLLISION, PH_CONVEX_QUEUE, PH_MAKE_CONSTRAINT, PH_WARMSTART,
+  PH_NEWTON_WAIT, PH_NEWTON_TRIPS, PH_NEWTON_ITERS, PH_MAKE_HESSIAN, PH_CHOL_FACTOR, PH_CHOL_SOLVE, PH_LINE_SEARCH, PH_LS_EVAL,
+  PH_LS_EVALS, PH_UPDATE_CONSTRAINT, PH_UPDATE_GRADIENT, PH_NEWTON_TAIL, PH_INTEGRATOR, PH_SUBSTEP, PH_SUBSTEPS, PH_PROLOGUE,
+  PH_EPILOGUE, PH_GROUPS, PH_N
+};
+#if defined(LOCOSIM_PHASE_CLOCK) && !defined(LS_EMULATE)
+#define LS_PH_SLOTS (256 * 16)
+__device__ unsigned long long g_phase[LS_PH_SLOTS][PH_N];
+__device__ __forceinline__ void ph_add(int ph, long long v) {
+  if ((threadIdx.x & 31) == 0) atomicAdd(&g_phase[(blockIdx.x & 255) * 16 + (threadIdx.x >> 5)][ph], (unsigned long long)v);
+}
+#define PH_T0(t) long long t = clock64()
+#define PH_LAP(ph, t) do { const long long n_ = clock64(); ph_add((ph), n_ - (t)); (t) = n_; } while (0)
+#define PH_CNT(ph, n) ph_add((ph), (n))
+#else
+#define PH_T0(t) ((void)0)
+#define PH_LAP(ph, t) ((void)0)
+#define PH_CNT(ph, n) ((void)0)
+#endif
+
 struct SolverOpts {
   float tolerance;     // Newton termination (scaled improvement / gradient), fp32-appropriate
   float ls_tolerance;  // relative line-search gradient tolerance
@@ -1600,6 +1624,7 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
     const int nw = (int)(blockDim.x >> 5);
     const int nj = nsurv < LS_MAXJOB ? nsurv : LS_MAXJOB;
     LANE0 { e.njobs = nj; }
+    PH_T0(t);
     __syncthreads();
     int incl = lane < nw ? blk[lane].njobs : 0;
     __syncthreads();        // (everybody has read the counts: a warp that runs ahead may publish its next evaluation's count)
@@ -1623,6 +1648,7 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
         convex_job(ms, o, e, (int)ocand[g - first], o.r_D + 8 * (g - first));
       }
       __syncthreads();
+      PH_LAP(PH_CONVEX_QUEUE, t);
       if (threadIdx.x == 0) blk[0].job_head = 0;       // (next use is behind the next evaluation's first barrier)
       // (3) owners consume their records in pair order
       NOUNROLL for (int j = 0; j < nj; j++) {
@@ -2026,16 +2052,37 @@ LS_FN void make_hessian_split(const int ms, EnvS<C>& e) {
   for (int k = 0; k < 12; k++) h[k] = (c0 + k < NV) ? e.M[row][c0 + k] : 0.0f;
   __syncwarp();
   const float* w = e.r_Jv + nunit;
-  NOUNROLL for (int r = 0; r < nrow; r++) {
-    const float wr = w[r];
-    if (wr == 0.0f) continue;                       // warp-uniform: satisfied / linear / cone rows
-    const float t = wr * e.J[r][row];
+  // The rows with w != 0 (quadratic zone; satisfied / linear / cone rows have w = 0), as a warp-uniform bit list in row
+  // order. The loop loads the next listed row's weight, column entry and chunks before the current row's FFMAs, so a row
+  // costs its FFMAs instead of a weight load, a branch and the row's loads in series. Same rows, same order, same fmaf
+  // chain per h[k] as a plain scan.
+  static_assert(E::MAXROW <= 64, "row list: two ballots");
+  unsigned long long rest =
+      (unsigned long long)__ballot_sync(0xffffffffu, lane < nrow && !(w[lane] == 0.0f)) |
+      (unsigned long long)__ballot_sync(0xffffffffu, lane + 32 < nrow && !(w[lane + 32] == 0.0f)) << 32;
+  if (rest) {
+    int r = __ffsll((long long)rest) - 1;
+    rest &= rest - 1;
+    float wr = w[r], jr = e.J[r][row];
     const float4* rp = reinterpret_cast<const float4*>(e.J[r]) + q0;
+    float4 v[3] = {rp[0], rp[1], rp[2]};
+    for (;;) {
+      const bool more = rest != 0;
+      r = more ? __ffsll((long long)rest) - 1 : r;   // (after the last row: a harmless reload of it)
+      rest &= rest - 1;
+      const float wn = w[r], jn = e.J[r][row];
+      const float4* rn = reinterpret_cast<const float4*>(e.J[r]) + q0;
+      const float4 vn[3] = {rn[0], rn[1], rn[2]};
+      const float t = wr * jr;
 #pragma unroll
-    for (int q = 0; q < 3; q++) {
-      const float4 v = rp[q];
-      h[4 * q] = fmaf(t, v.x, h[4 * q]); h[4 * q + 1] = fmaf(t, v.y, h[4 * q + 1]);
-      h[4 * q + 2] = fmaf(t, v.z, h[4 * q + 2]); h[4 * q + 3] = fmaf(t, v.w, h[4 * q + 3]);
+      for (int q = 0; q < 3; q++) {
+        h[4 * q] = fmaf(t, v[q].x, h[4 * q]); h[4 * q + 1] = fmaf(t, v[q].y, h[4 * q + 1]);
+        h[4 * q + 2] = fmaf(t, v[q].z, h[4 * q + 2]); h[4 * q + 3] = fmaf(t, v[q].w, h[4 * q + 3]);
+      }
+      if (!more) break;
+      wr = wn; jr = jn;
+#pragma unroll
+      for (int q = 0; q < 3; q++) v[q] = vn[q];
     }
   }
   // unit rows (frictionloss / joint limits) only touch the diagonal
@@ -2050,32 +2097,48 @@ LS_FN void make_hessian_split(const int ms, EnvS<C>& e) {
     for (int k = 0; k < 12; k++) if (c0 + k == row) h[k] += dsum;
   }
   if (C::CONE == 1) {
-    NOUNROLL for (int ci = 0; ci < e.ncon; ci++) {
+    // The contacts in the cone zone as a warp-uniform bit list in contact order (lane ci tests contact ci). A contact's
+    // rows (dim <= 6) are read into registers by fully unrolled, predicated loads that the compiler issues together, so
+    // the contact costs its arithmetic instead of one shared-memory round trip per row and loop. The expressions are
+    // those of make_hessian_wide with coneS[a] = sc[a], coneU[a] = cu[a].
+    static_assert(E::MAXCON <= 32, "cone list: one ballot");
+    unsigned cones = __ballot_sync(0xffffffffu, lane < e.ncon && e.r_state[nunit + e.con_row[lane]] == ST_CONE);
+    while (cones) {
+      const int ci = __ffs((int)cones) - 1;
+      cones &= cones - 1;
       const int r0 = nunit + e.con_row[ci];
-      if (e.r_state[r0] != ST_CONE) continue;
       const int dim = e.con_dim[ci], jr0 = r0 - nunit;
       const float mu = e.con_mu[ci];
-      float TT = 0;
-      NOUNROLL for (int j = 1; j < dim; j++) { float u = e.r_jar[r0 + j] * e.con_fri[ci][j - 1]; TT += u * u; }
-      const float N = e.r_jar[r0] * mu, T = sqrtf(TT), invT = 1.0f / T;
-      if (lane < dim) {
-        float sc = lane == 0 ? mu : e.con_fri[ci][lane - 1];
-        e.coneS[lane] = sc; e.coneU[lane] = e.r_jar[r0 + lane] * sc * invT;     // unit tangential direction U / T
+      float jar[6], sc[6], jc[6];
+#pragma unroll
+      for (int a = 0; a < 6; a++) {
+        jar[a] = a < dim ? e.r_jar[r0 + a] : 0.0f;
+        sc[a] = a == 0 ? mu : (a < dim ? e.con_fri[ci][a - 1] : 0.0f);
+        jc[a] = a < dim ? e.J[jr0 + a][row] : 0.0f;
       }
-      __syncwarp();
+      float TT = 0;
+#pragma unroll
+      for (int j = 1; j < 6; j++) if (j < dim) { float u = jar[j] * sc[j]; TT += u * u; }
+      const float N = jar[0] * mu, T = sqrtf(TT), invT = 1.0f / T;
+      float cu[6];                                                             // unit tangential direction U / T
+#pragma unroll
+      for (int a = 0; a < 6; a++) cu[a] = jar[a] * sc[a] * invT;
       const float Dm = e.r_D[r0] / fmaxf(LS_MINVAL, mu * mu * (1 + mu * mu));
       const float kk = mu * N * invT, c2 = mu * mu - kk;
       // Hc (jar space) = Dm S [ e0 e0^T - mu (e0 u^T + u e0^T) + (mu N / T) u u^T + c2 I_t ] S  with u = U / T (unit,
       // tangential only; no 1/T^3 factor, which overflows in fp32 for a vanishing tangential velocity), I_t tangential:
       // v = Hc p for this lane's column p_a = J[a][row] in O(dim), then H[row][:] += sum_b v_b J[b][:]
-      const float p0 = e.coneS[0] * e.J[jr0][row];
+      const float p0 = sc[0] * jc[0];
       float pU = 0;
-      NOUNROLL for (int a = 1; a < dim; a++) pU = fmaf(e.coneU[a], e.coneS[a] * e.J[jr0 + a][row], pU);
-      NOUNROLL for (int b2 = 0; b2 < dim; b2++) {
+#pragma unroll
+      for (int a = 1; a < 6; a++) if (a < dim) pU = fmaf(cu[a], sc[a] * jc[a], pU);
+#pragma unroll
+      for (int b2 = 0; b2 < 6; b2++) {
+        if (b2 >= dim) break;
         float vb;
         if (b2 == 0) vb = p0 - mu * pU;
-        else vb = e.coneU[b2] * (kk * pU - mu * p0) + c2 * e.coneS[b2] * e.J[jr0 + b2][row];
-        vb *= Dm * e.coneS[b2];
+        else vb = cu[b2] * (kk * pU - mu * p0) + c2 * sc[b2] * jc[b2];
+        vb *= Dm * sc[b2];
         const float4* rp = reinterpret_cast<const float4*>(e.J[jr0 + b2]) + q0;
 #pragma unroll
         for (int q = 0; q < 3; q++) {
@@ -2084,7 +2147,6 @@ LS_FN void make_hessian_split(const int ms, EnvS<C>& e) {
           h[4 * q + 2] = fmaf(vb, v.z, h[4 * q + 2]); h[4 * q + 3] = fmaf(vb, v.w, h[4 * q + 3]);
         }
       }
-      __syncwarp();
     }
   }
   // owners publish columns 0..11, helpers 12..NV-1 (their columns 8..11 duplicate the owner's values)
@@ -2096,7 +2158,9 @@ LS_FN void make_hessian_split(const int ms, EnvS<C>& e) {
     for (int k = 4; k < 12; k++) if (c0 + k < NV) e.H[row][c0 + k] = h[k];
   }
   __syncwarp();
+  PH_T0(t);
   chol_factor<NV, E::NVP>(ms, e.H);
+  PH_LAP(PH_CHOL_FACTOR, t);
 }
 
 // CUDA build, any nv <= 32: lane i accumulates the whole row i of H in registers
@@ -2179,7 +2243,9 @@ LS_FN void make_hessian_wide(const int ms, EnvS<C>& e) {
     for (int j = 0; j < NV; j++) e.H[lane][j] = h[j];
   }
   __syncwarp();
+  PH_T0(t);
   chol_factor<NV, E::NVP>(ms, e.H);
+  PH_LAP(PH_CHOL_FACTOR, t);
 }
 template <class C>
 LS_DEV void make_hessian(const int ms, EnvS<C>& e) {
@@ -2302,6 +2368,7 @@ LS_FN LSPoint ls_eval(const int ms, const EnvS<C>& e, const float* qg, float alp
 #if defined(LS_EMULATE)
   g_ls_evals++;
 #endif
+  PH_T0(t);
   const DevModel& m = c_models[ms];
   const int nefc = e.nefc;
   float c = 0, d1 = 0, d2 = 0;
@@ -2355,6 +2422,8 @@ LS_FN LSPoint ls_eval(const int ms, const EnvS<C>& e, const float* qg, float alp
   d2 += 2 * qg[2];
   if (d2 <= 0) d2 = LS_MINVAL;
   LSPoint p = {alpha, c, d1, d2};
+  PH_LAP(PH_LS_EVAL, t);
+  PH_CNT(PH_LS_EVALS, 1);
 #if defined(LS_EMULATE) && defined(LS_TRACE)
   printf("    ls_eval alpha %.6e cost %.9e d1 %.6e d2 %.6e (qg %.4e %.4e %.4e)\n", alpha, c, d1, d2, qg[0], qg[1], qg[2]);
 #endif
@@ -2444,6 +2513,7 @@ LS_FN void fwd_constraint(const int ms, EnvS<C>& e, const SolverOpts so) {
   const float scale = 1.0f / (PRM(meaninertia)[0] * (nv > 1 ? nv : 1));
   float gauss = 0, cost = 0, gn = 0;
   int iter = 0;
+  PH_T0(t);
   if (nefc == 0) {
     PAR_FOR(i, nv) { e.qacc[i] = e.qacc_smooth[i]; e.qfrc_constraint[i] = 0; }
     SYNC();
@@ -2483,27 +2553,35 @@ LS_FN void fwd_constraint(const int ms, EnvS<C>& e, const SolverOpts so) {
   // cost any more (the cost value has reached its fp32 resolution; further iterations only move noise).
   bool active = nefc > 0 && so.max_iter > 0 && scale * sqrtf(gn) >= so.tolerance;
   bool force_dirty = false;   // ls_prepare borrows r_force / r_aref of the elliptic rows
+  PH_LAP(PH_WARMSTART, t);
   while (BLOCK_ANY(so.sync_iters, active)) {
+    PH_LAP(PH_NEWTON_WAIT, t);
+    PH_CNT(PH_NEWTON_TRIPS, 1);
     // (warps whose env has converged keep passing the same barriers until the whole block is done)
     if (active) make_hessian(ms, e);
     BLOCK_SYNC(so.sync_phases & 64);
+    PH_LAP(PH_MAKE_HESSIAN, t);
     float alpha = 0;
     if (active) {
       chol_solve<EnvS<C>::NV, EnvS<C>::NVP>(e.H, e.Mgrad);
       PAR_FOR(i, EnvS<C>::NV) e.search[i] = i < nv ? -e.Mgrad[i] : 0.0f;   // (padding read by the unrolled J product)
       SYNC();
+      PH_LAP(PH_CHOL_SOLVE, t);
       alpha = line_search(ms, e, so, gauss, scale, cost);
       if (!(fabsf(alpha) <= 1e30f)) alpha = 0;      // never step to a non-finite point
       if (alpha == 0) { active = false; force_dirty = (C::CONE == 1); }
     }
     BLOCK_SYNC(so.sync_phases & 128);
+    PH_LAP(PH_LINE_SEARCH, t);
     if (active) {
       PAR_FOR(i, nv) { e.qacc[i] += alpha * e.search[i]; e.Ma[i] += alpha * e.Mv[i]; }
       PAR_FOR(r, nefc) e.r_jar[r] += alpha * e.r_Jv[r];
       SYNC();
       const float oldcost = cost;
       cost = update_constraint(ms, e, &gauss);
+      PH_LAP(PH_UPDATE_CONSTRAINT, t);
       gn = update_gradient(ms, e);
+      PH_LAP(PH_UPDATE_GRADIENT, t);
       iter++;
 #if defined(LS_EMULATE) && defined(LS_TRACE)
       printf("  it %2d alpha %.3e cost %.9e impr %.3e grad %.3e nefc %d\n", iter, alpha, cost, scale * (oldcost - cost),
@@ -2512,10 +2590,13 @@ LS_FN void fwd_constraint(const int ms, EnvS<C>& e, const SolverOpts so) {
       active = iter < so.max_iter && scale * sqrtf(gn) >= so.tolerance && cost < oldcost;
     }
   }
+  PH_LAP(PH_NEWTON_WAIT, t);                                  // (the barrier that ended the loop)
   if (force_dirty) cost = update_constraint(ms, e, &gauss);   // rare: restore efc_force for contact_forces()
   LANE0 { e.solver_iter = iter; e.iter_sum += iter; }
   PAR_FOR(i, nv) e.qacc_ws[i] = e.qacc[i];
   SYNC();
+  PH_LAP(PH_NEWTON_TAIL, t);
+  PH_CNT(PH_NEWTON_ITERS, iter);
 }
 
 // ----------------------------------------------------------------------------------------------------------
@@ -2528,17 +2609,24 @@ LS_FN void forward(const int ms, EnvS<C>& e, const SolverOpts so) {
 #if defined(LS_EMULATE)
   g_forward_evals++;
 #endif
+  PH_T0(t);
   kinematics(ms, e);
   BLOCK_SYNC(so.sync_phases & 2);
+  PH_LAP(PH_KINEMATICS, t);
   com_pos(ms, e);
+  PH_LAP(PH_COM_POS, t);
   crb_factor(ms, e);
   BLOCK_SYNC(so.sync_phases & 4);
+  PH_LAP(PH_CRB_FACTOR, t);
   smooth_forces(ms, e);        // last user of the smooth-dynamics scratch that the constraint rows overlay
   BLOCK_SYNC(so.sync_phases & 8);
+  PH_LAP(PH_SMOOTH_FORCES, t);
   collision(ms, e);
   BLOCK_SYNC(so.sync_phases & 16);
+  PH_LAP(PH_COLLISION, t);
   make_constraint(ms, e);
   BLOCK_SYNC(so.sync_phases & 32);
+  PH_LAP(PH_MAKE_CONSTRAINT, t);
   fwd_constraint(ms, e, so);
 }
 
@@ -2643,9 +2731,14 @@ template <class C>
 LS_FN void physics_substeps(const int ms, EnvS<C>& e, const SolverOpts so, int nsub, const int* grf_group, int n_grf) {
   const DevModel& m = c_models[ms];
   for (int k = 0; k < nsub; k++) {
+    PH_T0(t_sub);
     forward(ms, e, so);
+    PH_T0(t);
     if constexpr (C::RK4 == 1) rk4_step(ms, e, so); else euler_step(ms, e);
     if (n_grf > 0) contact_forces(ms, e, grf_group, n_grf);
+    PH_LAP(PH_INTEGRATOR, t);
+    PH_LAP(PH_SUBSTEP, t_sub);
+    PH_CNT(PH_SUBSTEPS, 1);
   }
 }
 
