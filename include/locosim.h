@@ -59,9 +59,11 @@ int locosim_reset_rows(locosim_t* h, const uint8_t* d_mask, const int32_t* d_tra
  *   d_action   [n_envs, action_dim] in [-1, 1]
  *   d_obs      [n_envs, obs_dim]   observation after the step (the terminal observation for envs with done=1)
  *   d_reward   [n_envs]
- *   d_done     [n_envs] uint8      absorbing flag (has_fallen, or non-finite state)
+ *   d_done     [n_envs] uint8      bit 0 = absorbing (has_fallen, or non-finite state); bit 1 (value 2) = truncated by a time
+ *                                  limit (locosim_set_time_limit; never set while both limits are off)
  *   d_next_obs [n_envs, obs_dim]   observation to act on next (== d_obs unless done, then the reset observation); may be NULL
- * auto_reset: 0 leaves terminated envs in their terminal state (caller resets with locosim_reset). */
+ * auto_reset: 0 leaves terminated envs in their terminal state (caller resets with locosim_reset); truncated envs are
+ * auto-reset exactly like terminated ones. */
 int locosim_step(locosim_t* h, const float* d_action, float* d_obs, float* d_reward, uint8_t* d_done, float* d_next_obs,
                  int auto_reset, void* stream);
 
@@ -74,8 +76,40 @@ int locosim_set_state(locosim_t* h, const float* d_qpos, const float* d_qvel, co
  * counter-based draw, which is also what in-kernel auto-resets use). Requires a TaskSpec with TKI_ROT_* set. */
 int locosim_set_reset_rotation(locosim_t* h, const float* d_angle);
 
-/* Trajectory cursor of every env (traj * traj_len + sample; LS_REWARD_TRACKING, include/locosim_task.h). int32 [n_envs]. */
+/* Trajectory cursor of every env (traj * traj_len + sample; LS_REWARD_TRACKING and end_of_trajectory, include/locosim_task.h).
+ * int32 [n_envs]. */
 int locosim_get_cursor(locosim_t* h, int32_t* d_out, void* stream);
+
+/* Time limit: ends episodes that neither fall nor diverge. The reference leaves this to its consumer (mushroom Core enforces
+ * MDPInfo.horizon, and resets when Trajectory.get_next_sample() returns None: utils/trajectory.py:311-323, base.py:365-368);
+ * a batched loop relies on the in-kernel auto-reset, so the engine enforces it. An engine setting like locosim_set_solver
+ * (not part of the TaskSpec: one compiled task serves training with and evaluation without a limit). 0, 0 = off = the state
+ * after locosim_create; negative values are an error. Takes effect from the next locosim_step.
+ *
+ * Episode length = control steps since the env's last reset of any kind (locosim_reset*, in-kernel auto-reset);
+ * locosim_set_state does not restart it. Two independent limits:
+ *   max_episode_steps = H > 0: the episode is truncated by the control step that makes its length reach H.
+ *   end_of_trajectory = 1:     the trajectory cursor advances by one sample per control step under EVERY reward type (one
+ *       advance per step; LS_REWARD_TRACKING compares against the row at the advanced cursor as always), and the episode
+ *       is truncated by the step after which the cursor stands on the LAST sample of its trajectory: the step for which
+ *       get_next_sample() would next return None, i.e. the last step whose tracking reward has a table row of its own.
+ *       An episode reset to sample s of a trajectory of traj_len samples is therefore truncated by its step number
+ *       traj_len - 1 - s (s = traj_len - 3: second step, s = traj_len - 2: first step). An episode reset ONTO the last
+ *       sample cannot advance: its first step is truncated and the cursor stays where it is.
+ *       With the option off the cursor moves under LS_REWARD_TRACKING only and is clamped at the last sample.
+ * Absorbing wins: a step that is terminal and at a limit reports bit 0 only. With auto_reset = 1 a truncated env is reset in
+ * the same step like a fallen one (d_obs = the final observation of the old episode, d_next_obs = the reset observation;
+ * episode counter, pool row, goal, rotation, cursor and LOCOSIM_KEY_RESET as for any auto-reset). With auto_reset = 0 bit 1
+ * is reported on that step and on every later step until the caller resets the env; nothing else changes. */
+int locosim_set_time_limit(locosim_t* h, int max_episode_steps, int end_of_trajectory);
+
+/* Per-episode statistics, kept per env on the device whether or not a limit is set: d_len int32 / d_ret fp32 = control steps
+ * and sum of the rewards locosim_step wrote (fp32, in step order) of the RUNNING episode (both 0 after a reset); d_last_len /
+ * d_last_ret = the same two of the env's last FINISHED episode (finished = a step reported absorbing or truncated; 0 before
+ * the first one; an env that stays finished under auto_reset = 0 rewrites them every step). Rewards evaluated outside the
+ * engine (LS_REWARD_NONE, the Python facade's reward_type="custom") count as the 0 the engine writes. Each [n_envs], each
+ * may be NULL; stream-ordered copies like locosim_get_cursor. */
+int locosim_get_episode_stats(locosim_t* h, int32_t* d_len, float* d_ret, int32_t* d_last_len, float* d_last_ret, void* stream);
 
 /* Replaces LocoEnv.create_dataset() (base.py:278-312 -> utils/trajectory.py:104-151) on the device: consecutive samples of
  * every trajectory of the reset table in observation layout. d_states / d_next_states fp32 [locosim_dataset_rows, obs_dim],

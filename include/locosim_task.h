@@ -66,7 +66,9 @@ enum {
   /* Mocap-tracking reward (BASELINE config 3 "imitation reward vs mocap dataset"). NOT in the reference (none of its six
    * rewards reads the trajectory, SURVEY F7): this package's own spec, DeepMimic-style. Every env carries a trajectory
    * cursor (traj, sample), set by each (auto-)reset to the sampled reset row and advanced by one sample per control
-   * step (clamped at the last sample). With P / V = the observation entries gathered from qpos / qvel,
+   * step (clamped at the last sample; with the engine setting end_of_trajectory, include/locosim.h locosim_set_time_limit,
+   * the cursor advances under every reward type and the step that puts it on the last sample truncates the episode, so no
+   * two steps of an episode are rewarded against the same row). With P / V = the observation entries gathered from qpos / qvel,
    *   r = wp * exp(-kp * sum_{k in P} (obs[k] - ref[k])^2) + wv * exp(-kv * sum_{k in V} (obs[k] - ref[k])^2),
    * evaluated on the observation AFTER the step against the table row at the advanced cursor (the reward of the step
    * that reached it; the observation's root x / y are not part of it). */

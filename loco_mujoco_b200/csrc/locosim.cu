@@ -27,7 +27,10 @@ struct EngineState {
   int* counters;                    // [N,8]
   int* dr_row;                      // [N] row of the parameter pool used by the env's current episode
   int* perm;                        // [N] env handled by warp slot i (regrouped every step by solver effort)
-  int* cursor;                      // [N] trajectory cursor traj * traj_len + sample (LS_REWARD_TRACKING)
+  int* cursor;                      // [N] trajectory cursor traj * traj_len + sample (LS_REWARD_TRACKING, end_of_trajectory)
+  int4* ep;                         // [N] episode statistics: x = control steps, y = sum of the written rewards (fp32 bits) since the
+                                    // env's last reset; z, w = the same two of its last finished (absorbing or truncated) episode
+  int max_episode_steps, end_of_trajectory;   // time limit (locosim_set_time_limit), 0 = off
   const float* rot_angle;           // [N] rotation angles pinned for the next reset (setup_random_rot, drop-in mode) or NULL
   const float* pool;                // [K, P] parameter pool (domain randomisation); K = 1: the model's own values
   int pool_K;
@@ -103,6 +106,7 @@ __global__ void reset_kernel(int ms, DevTask t, EngineState st, const uint8_t* m
     st.episode[env] = ep + 1; st.counters[(size_t)env * 8 + 1] += 1;
     st.dr_row[env] = prow;
     st.cursor[env] = tr * t.traj_len + sp;
+    *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
   }
 }
 #endif
@@ -283,10 +287,26 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
     if (bad) v = 0.0f;
     obs[(size_t)env * D + k] = v;
   }
+  bool truncated = false;
   if (lane == 0) {
     float r = rew;
     reward[env] = r;
-    done[env] = is_done ? 1 : 0;
+    // episode statistics and time limit (include/locosim.h): length and return of the running episode, the two limits,
+    // bit 1 of the done byte (absorbing wins), the finished episode's numbers
+    int4 es = st.ep[env];
+    es.x += 1; es.y = __float_as_int(__int_as_float(es.y) + r);
+    truncated = st.max_episode_steps > 0 && es.x >= st.max_episode_steps;
+    if (st.end_of_trajectory) {
+      // one (clamped) advance of the cursor per step: the tracking reward above has made it already
+      const int cur = st.cursor[env];
+      int sp = cur % t.traj_len;
+      if (t.reward_type != LS_REWARD_TRACKING && sp + 1 < t.traj_len) { sp += 1; st.cursor[env] = cur + 1; }
+      truncated |= sp == t.traj_len - 1;
+    }
+    truncated = truncated && !is_done;
+    done[env] = is_done ? 1 : (truncated ? 2 : 0);
+    if (is_done || truncated) { es.z = es.x; es.w = es.y; }
+    st.ep[env] = es;
     int* cnt = st.counters + (size_t)env * 8;
     cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
     if (bad) cnt[4] += 1;
@@ -305,8 +325,9 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
     } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
   }
 
-  // ---- auto-reset ----
-  if (is_done && (auto_reset || bad)) {
+  // ---- auto-reset (reset_env is a whole-warp call: lane 0's verdict on the time limit goes to every lane first) ----
+  truncated = __shfl_sync(0xffffffffu, (int)truncated, 0) != 0;
+  if ((is_done || truncated) && (auto_reset || bad)) {
     const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
     int ep = st.episode[env];
     int tr, sp;
@@ -319,6 +340,7 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
       if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
       st.dr_row[env] = prow;
       st.cursor[env] = tr * t.traj_len + sp;
+      *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
       e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
     }
     __syncwarp();
@@ -490,10 +512,26 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
     if (bad) v = 0.0f;
     obs[(size_t)env * D + k] = v;
   }
+  bool truncated = false;
   if (lane == 0) {
     float r = rew;
     reward[env] = r;
-    done[env] = is_done ? 1 : 0;
+    // episode statistics and time limit (include/locosim.h): length and return of the running episode, the two limits,
+    // bit 1 of the done byte (absorbing wins), the finished episode's numbers
+    int4 es = st.ep[env];
+    es.x += 1; es.y = __float_as_int(__int_as_float(es.y) + r);
+    truncated = st.max_episode_steps > 0 && es.x >= st.max_episode_steps;
+    if (st.end_of_trajectory) {
+      // one (clamped) advance of the cursor per step: the tracking reward above has made it already
+      const int cur = st.cursor[env];
+      int sp = cur % t.traj_len;
+      if (t.reward_type != LS_REWARD_TRACKING && sp + 1 < t.traj_len) { sp += 1; st.cursor[env] = cur + 1; }
+      truncated |= sp == t.traj_len - 1;
+    }
+    truncated = truncated && !is_done;
+    done[env] = is_done ? 1 : (truncated ? 2 : 0);
+    if (is_done || truncated) { es.z = es.x; es.w = es.y; }
+    st.ep[env] = es;
     int* cnt = st.counters + (size_t)env * 8;
     cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
     if (bad) cnt[4] += 1;
@@ -512,8 +550,9 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
     } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
   }
 
-  // ---- auto-reset ----
-  if (is_done && (auto_reset || bad)) {
+  // ---- auto-reset (reset_env is a whole-warp call: lane 0's verdict on the time limit goes to every lane first) ----
+  truncated = __shfl_sync(0xffffffffu, (int)truncated, 0) != 0;
+  if ((is_done || truncated) && (auto_reset || bad)) {
     const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
     int ep = st.episode[env];
     int tr, sp;
@@ -526,6 +565,7 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
       if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
       st.dr_row[env] = prow;
       st.cursor[env] = tr * t.traj_len + sp;
+      *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
       e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
     }
     __syncwarp();
@@ -541,7 +581,7 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
   }
   if (lane == 0 && split.regroup) {
     int key = launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in);
-    if (is_done && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
+    if ((is_done || truncated) && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
     append_env(split, rd ^ 1, env, n_envs, key);
   }
 }
@@ -834,10 +874,26 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
     if (bad) v = 0.0f;
     obs[(size_t)env * D + k] = v;
   }
+  bool truncated = false;
   if (lane == 0) {
     float r = rew;
     reward[env] = r;
-    done[env] = is_done ? 1 : 0;
+    // episode statistics and time limit (include/locosim.h): length and return of the running episode, the two limits,
+    // bit 1 of the done byte (absorbing wins), the finished episode's numbers
+    int4 es = st.ep[env];
+    es.x += 1; es.y = __float_as_int(__int_as_float(es.y) + r);
+    truncated = st.max_episode_steps > 0 && es.x >= st.max_episode_steps;
+    if (st.end_of_trajectory) {
+      // one (clamped) advance of the cursor per step: the tracking reward above has made it already
+      const int cur = st.cursor[env];
+      int sp = cur % t.traj_len;
+      if (t.reward_type != LS_REWARD_TRACKING && sp + 1 < t.traj_len) { sp += 1; st.cursor[env] = cur + 1; }
+      truncated |= sp == t.traj_len - 1;
+    }
+    truncated = truncated && !is_done;
+    done[env] = is_done ? 1 : (truncated ? 2 : 0);
+    if (is_done || truncated) { es.z = es.x; es.w = es.y; }
+    st.ep[env] = es;
     int* cnt = st.counters + (size_t)env * 8;
     cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
     if (bad) cnt[4] += 1;
@@ -856,8 +912,9 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
     } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
   }
 
-  // ---- auto-reset ----
-  if (is_done && (auto_reset || bad)) {
+  // ---- auto-reset (reset_env is a whole-warp call: lane 0's verdict on the time limit goes to every lane first) ----
+  truncated = __shfl_sync(0xffffffffu, (int)truncated, 0) != 0;
+  if ((is_done || truncated) && (auto_reset || bad)) {
     const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
     int ep = st.episode[env];
     int tr, sp;
@@ -870,6 +927,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
       if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
       st.dr_row[env] = prow;
       st.cursor[env] = tr * t.traj_len + sp;
+      *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
       e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
     }
     __syncwarp();
@@ -888,7 +946,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
   if (lane == 0) {
     // into chunk 0 of the next step
     int key = launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in);
-    if (is_done && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
+    if ((is_done || truncated) && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
     persist_publish(q, par, q.nch, env, n_envs, key);
   }
   PH_LAP(PH_EPILOGUE, t_epi);
@@ -1280,11 +1338,14 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
        cudaMalloc((void**)&h->st.episode, N * 4) == cudaSuccess && cudaMalloc((void**)&h->st.counters, N * 32) == cudaSuccess &&
        cudaMalloc((void**)&h->st.dr_row, N * 4) == cudaSuccess && cudaMalloc((void**)&h->st.perm, N * 4) == cudaSuccess &&
        cudaMalloc((void**)&h->st.cursor, N * 4) == cudaSuccess &&
+       cudaMalloc((void**)&h->st.ep, N * 16) == cudaSuccess &&
        up((void**)&h->d_pool, h->hm.default_row.data(), h->hm.default_row.size() * 4);
   if (!ok) { std::string m = std::string("device allocation failed: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); g_create_error = m; return 1; }
   cudaMemset(h->st.qpos, 0, N * nv * 4); cudaMemset(h->st.qvel, 0, N * nv * 4); cudaMemset(h->st.ws, 0, N * nv * 4);
   cudaMemset(h->st.goal, 0, N * 16); cudaMemset(h->st.episode, 0, N * 4); cudaMemset(h->st.counters, 0, N * 32);
   cudaMemset(h->st.dr_row, 0, N * 4); cudaMemset(h->st.cursor, 0, N * 4);
+  cudaMemset(h->st.ep, 0, N * 16);
+  h->st.max_episode_steps = 0; h->st.end_of_trajectory = 0;
   h->st.rot_angle = nullptr;
   { std::vector<int> id(N); for (size_t i = 0; i < N; i++) id[i] = (int)i; cudaMemcpy(h->st.perm, id.data(), N * 4, cudaMemcpyHostToDevice); }
   h->st.pool = h->d_pool; h->st.pool_K = 1;
@@ -1323,6 +1384,7 @@ void locosim_destroy(locosim_t* h) {
   cudaFree(h->d_mints); cudaFree(h->d_mreals); cudaFree(h->d_tints); cudaFree(h->d_treals);
   cudaFree(h->st.qpos); cudaFree(h->st.qvel); cudaFree(h->st.ws); cudaFree(h->st.goal); cudaFree(h->st.episode);
   cudaFree(h->st.counters); cudaFree(h->st.dr_row); cudaFree(h->st.perm); cudaFree(h->st.cursor); cudaFree(h->d_pool);
+  cudaFree(h->st.ep);
   cudaFree(h->d_stage);
   cudaFree(h->split.carry); cudaFree(h->split.bcount); cudaFree(h->split.benv); cudaFree(h->split.seq);
   cudaFree(h->pq.carry); cudaFree(h->pq.cnt); cudaFree(h->pq.tot); cudaFree(h->pq.benv); cudaFree(h->pq.seq);
@@ -1353,6 +1415,19 @@ int locosim_reset_rows(locosim_t* h, const uint8_t* d_mask, const int32_t* d_tra
 int locosim_set_reset_rotation(locosim_t* h, const float* d_angle) { h->st.rot_angle = d_angle; return 0; }
 int locosim_get_cursor(locosim_t* h, int32_t* d_out, void* stream) {
   CK(cudaMemcpyAsync(d_out, h->st.cursor, (size_t)h->n_envs * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+int locosim_set_time_limit(locosim_t* h, int max_episode_steps, int end_of_trajectory) {
+  if (max_episode_steps < 0 || end_of_trajectory < 0) { h->err = "bad time limit (negative)"; return 1; }
+  h->st.max_episode_steps = max_episode_steps; h->st.end_of_trajectory = end_of_trajectory ? 1 : 0;
+  return 0;
+}
+int locosim_get_episode_stats(locosim_t* h, int32_t* d_len, float* d_ret, int32_t* d_last_len, float* d_last_ret, void* stream) {
+  // (one 16-byte record per env on the device: four strided copies)
+  void* dst[4] = {d_len, d_ret, d_last_len, d_last_ret};
+  for (int k = 0; k < 4; k++)
+    if (dst[k]) CK(cudaMemcpy2DAsync(dst[k], 4, (const char*)h->st.ep + 4 * k, 16, 4, (size_t)h->n_envs, cudaMemcpyDeviceToDevice,
+                                     (cudaStream_t)stream));
   return 0;
 }
 

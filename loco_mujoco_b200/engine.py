@@ -74,6 +74,10 @@ def load_library():
     lib.locosim_launch_info.argtypes = [vp, ctypes.POINTER(ip), ctypes.POINTER(ip), ctypes.POINTER(ip)]
     lib.locosim_set_timeline.restype = ip
     lib.locosim_set_timeline.argtypes = [vp, vp, ip]
+    lib.locosim_set_time_limit.restype = ip
+    lib.locosim_set_time_limit.argtypes = [vp, ip, ip]
+    lib.locosim_get_episode_stats.restype = ip
+    lib.locosim_get_episode_stats.argtypes = [vp, vp, vp, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -84,7 +88,16 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_param_pool_row_len", "locosim_set_param_pool", "locosim_get_param_rows",
                     "locosim_kernels_per_step", "locosim_reset_rows", "locosim_set_goal", "locosim_measure_fp32_peak",
                     "locosim_set_reset_rotation", "locosim_get_cursor", "locosim_dataset_rows", "locosim_create_dataset",
-                    "locosim_debug_counters", "locosim_set_timeline"]
+                    "locosim_debug_counters", "locosim_set_timeline", "locosim_set_time_limit",
+                    "locosim_get_episode_stats"]
+
+# bits of the done byte of a step (include/locosim.h)
+DONE_ABSORBING, DONE_TRUNCATED = 1, 2
+
+
+def split_done(done):
+    """done bytes of a step -> (absorbing, truncated) bool masks (torch or numpy uint8 in, the same kind out)."""
+    return (done & DONE_ABSORBING) != 0, (done & DONE_TRUNCATED) != 0
 
 
 def measure_fp32_peak(device=0):
@@ -197,7 +210,8 @@ class CudaEngine:
         return self.n_envs * (4 * self.obs_dim + 5)
 
     def step(self, action, auto_reset=True, want_next_obs=True, packed=None):
-        """action: float32 cuda [n_envs, action_dim] (contiguous). Returns (obs, reward, done, next_obs) views.
+        """action: float32 cuda [n_envs, action_dim] (contiguous). Returns (obs, reward, done, next_obs) views; `done` is the
+        engine's byte (bit 0 absorbing, bit 1 truncated by `set_time_limit`: `split_done`).
         packed: optional uint8 cuda buffer of `packed_bytes` (16-byte aligned, e.g. one time slot of a rollout buffer)
         the kernel writes this step's obs / reward / done into instead of the engine's own `packed_out`."""
         if action.dtype != self.torch.float32 or not action.is_contiguous() or action.device != self.device:
@@ -230,6 +244,20 @@ class CudaEngine:
             if x is not None and (x.dtype != self.torch.float32 or not x.is_contiguous()):
                 raise ValueError("state tensors must be contiguous float32")
         self._check(self.lib.locosim_set_state(self.h, _ptr(qpos), _ptr(qvel), _ptr(qacc_warmstart), self._stream()))
+
+    def set_time_limit(self, max_episode_steps=0, end_of_trajectory=False):
+        """Time limit of include/locosim.h: truncate an episode at `max_episode_steps` control steps (0 = no limit) and / or
+        where its trajectory cursor reaches the last mocap sample. Reported as bit 1 of `done`; takes effect from the next step."""
+        self._check(self.lib.locosim_set_time_limit(self.h, int(max_episode_steps), int(bool(end_of_trajectory))))
+
+    def episode_stats(self):
+        """(length int32, return float32, last_length, last_return), each [n_envs]: the running episode's control steps and
+        summed engine rewards, and those of the env's last finished (absorbing or truncated) episode."""
+        t = self.torch
+        ln, last_ln = (t.empty((self.n_envs,), dtype=t.int32, device=self.device) for _ in range(2))
+        ret, last_ret = (t.empty((self.n_envs,), dtype=t.float32, device=self.device) for _ in range(2))
+        self._check(self.lib.locosim_get_episode_stats(self.h, _ptr(ln), _ptr(ret), _ptr(last_ln), _ptr(last_ret), self._stream()))
+        return ln, ret, last_ln, last_ret
 
     def cursor(self):
         t = self.torch

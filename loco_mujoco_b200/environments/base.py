@@ -23,6 +23,7 @@ from itertools import product
 import numpy as np
 
 from .. import mjcf, modelpack
+from ..engine import DONE_ABSORBING, DONE_TRUNCATED, split_done
 from ..task import (TaskSpec, OBS_QPOS, OBS_QVEL, OBS_GOAL, OBS_GRF, OBS_PARAM, GRF_FLOOR, REWARD_NONE, REWARD_TARGET_VELOCITY,
                     REWARD_POS, REWARD_TRACKING)
 from ..trajectory import Trajectory
@@ -123,6 +124,19 @@ def reference_data_root():
     return None
 
 
+def resolve_time_limit(time_limit, horizon):
+    """`time_limit` argument of LocoEnv -> max_episode_steps of the engine (0 = no limit)."""
+    if time_limit is None:
+        return 0
+    if isinstance(time_limit, str):
+        if time_limit != "horizon":
+            raise ValueError("time_limit must be None, a positive number of control steps or \"horizon\", not %r" % (time_limit,))
+        time_limit = horizon
+    if isinstance(time_limit, bool) or int(time_limit) != time_limit or time_limit <= 0:
+        raise ValueError("time_limit must be a positive number of control steps, not %r" % (time_limit,))
+    return int(time_limit)
+
+
 ASSET_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "assets")
 
 
@@ -148,7 +162,8 @@ class LocoEnv:
                  init_step_no=None, timestep=0.001, use_foot_forces=False, default_camera_mode="follow",
                  use_absorbing_states=True, domain_randomization_config=None, parallel_dom_rand=True,
                  N_worker_per_xml_dom_rand=4, num_envs=None, device="cuda:0", seed=0, env_id_offset=0,
-                 compiled_model=None, copy_outputs=True, convex_collisions=True, warps_per_block=None, **viewer_params):
+                 compiled_model=None, copy_outputs=True, convex_collisions=True, warps_per_block=None, time_limit=None,
+                 truncate_at_trajectory_end=False, **viewer_params):
         if type(xml_handles) != list:
             xml_handles = [xml_handles]
         self._xml_handles = xml_handles
@@ -214,8 +229,18 @@ class LocoEnv:
         self._convex_collisions = bool(convex_collisions)
         # launch geometry of the step kernel (envs per block); None = the engine's choice. Scheduling only (MixedBatch uses it)
         self._warps_per_block = warps_per_block
+        # Time limit (include/locosim.h locosim_set_time_limit), off by default like in the reference, whose env never
+        # truncates (there the consumer enforces `horizon`): time_limit = None, a number of control steps, or "horizon" (= the
+        # `horizon` argument); truncate_at_trajectory_end ends an episode where its mocap trajectory does. With either on,
+        # step() reports `info["truncated"]`, and batched envs reset truncated episodes in the same step like fallen ones.
+        self._max_episode_steps = resolve_time_limit(time_limit, horizon)
+        self._truncate_at_trajectory_end = bool(truncate_at_trajectory_end)
         self._engine = None
         self._obs = None
+
+    @property
+    def time_limited(self):
+        return self._max_episode_steps > 0 or self._truncate_at_trajectory_end
 
     # ---------------------------------------------------------------------------------------------------
     # construction helpers
@@ -398,6 +423,8 @@ class LocoEnv:
                 self._engine.set_param_pool(self.domain_randomization_pool())
             elif len(self._models) > 1 or len(self._model_user_features[0]):
                 self._engine.set_param_pool(self.model_pool())
+            if self.time_limited:
+                self._engine.set_time_limit(self._max_episode_steps, self._truncate_at_trajectory_end)
         return self._engine
 
     # ---------------------------------------------------------------------------------------------------
@@ -506,13 +533,15 @@ class LocoEnv:
             a = torch.as_tensor(np.asarray(action, dtype=np.float32).reshape(1, -1), device=eng.device)
             obs, reward, done, _ = eng.step(a.contiguous(), auto_reset=False, want_next_obs=False)
             cur = obs[0].double().cpu().numpy()
-            absorbing = bool(done[0].item())
+            flags = int(done[0].item())
+            absorbing = bool(flags & DONE_ABSORBING)
             if self._reward_type == "custom":
                 r = self._reward_function(self._obs, np.asarray(action), cur, absorbing)
             else:
                 r = float(reward[0].item())
             self._obs = cur
-            return cur.copy(), r, absorbing, {}
+            # (no auto-reset in this mode: a truncated episode is reset by the caller, as in the reference)
+            return cur.copy(), r, absorbing, ({"truncated": bool(flags & DONE_TRUNCATED)} if self.time_limited else {})
         if action.dtype != torch.float32:
             action = action.float()
         prev = self._obs
@@ -529,6 +558,12 @@ class LocoEnv:
             cb = self._reward_function._reward_callback
             reward = cb(prev, action, obs) if cb is not None else torch.zeros_like(reward)
         self._obs = next_obs
+        if self.time_limited:
+            # `done` keeps its meaning (absorbing); the last finished episode's length and return are valid where
+            # done | truncated (the return sums the ENGINE's rewards: 0 under reward_type="custom")
+            done, info["truncated"] = split_done(done)
+            _, _, info["episode_length"], info["episode_return"] = eng.episode_stats()
+            return obs, reward, done, info
         return obs, reward, done.view(torch.bool), info      # (0/1 bytes reinterpreted, no kernel)
 
     def is_absorbing(self, obs):

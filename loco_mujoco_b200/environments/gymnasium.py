@@ -32,7 +32,8 @@ except Exception:                       # gymnasium is not installed in the buil
 
 
 class GymnasiumWrapper(_Base):
-    """step -> (obs, reward, terminated, truncated=False, info); reset(seed, options) -> (obs, {})."""
+    """step -> (obs, reward, terminated, truncated, info); reset(seed, options) -> (obs, {}). `truncated` is False unless the
+    env was made with `time_limit` / `truncate_at_trajectory_end` (LocoEnv); the caller resets a truncated env."""
 
     metadata = {"render_modes": ["human", "rgb_array"], "render_fps": 100}
 
@@ -46,7 +47,7 @@ class GymnasiumWrapper(_Base):
 
     def step(self, action):
         obs, reward, absorbing, info = self._env.step(action)
-        return obs, reward, absorbing, False, info
+        return obs, reward, absorbing, info.get("truncated", False), info
 
     def reset(self, *, seed=None, options=None):
         if seed is not None and _gym is not None:
@@ -80,11 +81,16 @@ class VectorGymnasiumWrapper:
     """Batched counterpart with the Gymnasium VectorEnv call contract (SURVEY 8(f).4): `num_envs` independent copies on
     one GPU, autoreset in the same step ("SAME_STEP" mode: for sub-envs that terminated, `obs` is already the first
     observation of the next episode and `info["final_obs"]` holds the terminal observation of ALL sub-envs, to be
-    masked with `terminated`). Tensors stay on the device (torch.cuda) unless `to_numpy=True`.
+    masked with `terminated | truncated`). `time_limit` / `truncate_at_trajectory_end` (LocoEnv keyword arguments) turn the
+    time limit on: `truncated` is then the engine's flag, and `info["episode"] = {"r": return, "l": length}` with the mask
+    `info["_episode"]` reports the episodes that ended in this step (the keys of Gymnasium's RecordEpisodeStatistics).
+    Tensors stay on the device (torch.cuda) unless `to_numpy=True`.
     The reference has no vector interface; its single-env wrapper is `GymnasiumWrapper` (gymnasium.py:11-173)."""
 
-    def __init__(self, env_name, num_envs, device="cuda:0", seed=0, to_numpy=False, **kwargs):
-        self._env = LocoEnv.make(env_name, num_envs=num_envs, device=device, seed=seed, **kwargs)
+    def __init__(self, env_name, num_envs, device="cuda:0", seed=0, to_numpy=False, time_limit=None,
+                 truncate_at_trajectory_end=False, **kwargs):
+        self._env = LocoEnv.make(env_name, num_envs=num_envs, device=device, seed=seed, time_limit=time_limit,
+                                 truncate_at_trajectory_end=truncate_at_trajectory_end, **kwargs)
         self.num_envs = int(num_envs)
         self._to_numpy = to_numpy
         one_obs, one_act = self._env.info.observation_space, self._env.info.action_space
@@ -107,9 +113,14 @@ class VectorGymnasiumWrapper:
         if not torch.is_tensor(actions):
             actions = torch.as_tensor(np.asarray(actions, dtype=np.float32), device=self._env._get_engine().device)
         obs, reward, done, info = self._env.step(actions)
-        truncated = torch.zeros_like(done)
-        return (self._out(info["next_obs"]), self._out(reward), self._out(done), self._out(truncated),
-                {"final_obs": self._out(obs)})
+        out = {"final_obs": self._out(obs)}
+        if "truncated" in info:
+            truncated = info["truncated"]
+            out["episode"] = {"r": self._out(info["episode_return"]), "l": self._out(info["episode_length"])}
+            out["_episode"] = self._out(done | truncated)
+        else:
+            truncated = torch.zeros_like(done)
+        return self._out(info["next_obs"]), self._out(reward), self._out(done), self._out(truncated), out
 
     def close(self):
         self._env.stop()

@@ -324,7 +324,8 @@ class HumanoidTorque4AgesAll:
             return self.subs[self._current_model_idx].step(action)
         outs = [s.step(action[k::4].contiguous()) for k, s in enumerate(self.subs)]
         obs, rew, done = (self._scatter([o[j] for o in outs]) for j in range(3))
-        return obs, rew, done, {"next_obs": self._scatter([o[3]["next_obs"] for o in outs])}
+        # (every info entry is a per-env tensor: next_obs, and with a time limit truncated / episode_length / episode_return)
+        return obs, rew, done, {k: self._scatter([o[3][k] for o in outs]) for k in outs[0][3]}
 
     def create_dataset(self, ignore_keys=None):
         """The four humanoids' datasets, concatenated in scaling order (the layout of the reference's `_all` dataset)."""

@@ -131,6 +131,10 @@ class MixedBatch:
     (`balance=True`) and the slowest one gets the high-priority stream: its blocks are dispatched first whenever both
     kernels have blocks pending; the lighter members run in full blocks (two spread kernels sharing every SM still hit the slow
     mode in 1 of 4 runs, spread + full blocks in 0 of 8).
+
+    `time_limit` / `truncate_at_trajectory_end` (LocoEnv keyword arguments, for all members through `**common` or per member)
+    reach every member's engine. `step` returns the engines' own tuples, so `done` is the byte of include/locosim.h:
+    `engine.split_done(done)` gives the absorbing and truncated masks, `engines[i].episode_stats()` the episode numbers.
     """
 
     def __init__(self, members, device="cuda:0", seed=0, env_id_offset=0, concurrent=True, balance=True, stagger_us=40.0, **common):
