@@ -111,6 +111,27 @@ int locosim_set_time_limit(locosim_t* h, int max_episode_steps, int end_of_traje
  * may be NULL; stream-ordered copies like locosim_get_cursor. */
 int locosim_get_episode_stats(locosim_t* h, int32_t* d_len, float* d_ret, int32_t* d_last_len, float* d_last_ret, void* stream);
 
+/* Bodies of the compiled model, the world (body 0) included: the row length of the xfrc_applied buffer below is 6 * nbody.
+ * Body indices are those of the compiled model (fuse_static merges static bodies into their parents). */
+int locosim_nbody(const locosim_t* h);
+
+/* Applied forces, MuJoCo 2.3.7's mjData.xfrc_applied / qfrc_applied (how a loco-mujoco user pushes a robot through
+ * env._data): caller-owned DEVICE buffers, registered once and read by every later locosim_step.
+ *   d_xfrc fp32 [n_envs, nbody, 6]: per body a force (3) then a torque (3), world coordinates, applied at the body's centre
+ *          of mass (xipos), as mj_applyFT does. Row 0 (the world) is ignored.
+ *   d_qfrc fp32 [n_envs, nq]:       generalised forces.
+ * Either may be NULL; NULL, NULL = off = the state after locosim_create (nothing is read then, and no output changes by a bit).
+ * Semantics of mj_fwdAcceleration + mj_xfrcAccumulate: qfrc_smooth = passive - bias + actuator + qfrc_applied
+ * + sum over bodies of J_b^T xfrc_applied[b], in EVERY dynamics evaluation with that evaluation's kinematics (Euler: once per
+ * sub-step; RK4: each of the four stages); the constraint solver sees them through qacc_smooth.
+ * They last until the caller changes them: the engine only writes zeros, into the rows of every env it resets (locosim_reset*
+ * for the masked envs, the in-kernel auto-reset for the envs it resets), as mj_resetData does; locosim_set_state leaves them
+ * alone. So the buffers must stay valid and writable while registered. An engine setting like locosim_set_time_limit (not
+ * part of the TaskSpec); takes effect from the next locosim_step. The pointers are engine state, not per-call values: register
+ * them outside of stream capture (before cudaStreamBeginCapture); a captured step then reads whatever the buffers hold when
+ * it is replayed. */
+int locosim_set_applied_forces(locosim_t* h, float* d_xfrc, float* d_qfrc);
+
 /* Replaces LocoEnv.create_dataset() (base.py:278-312 -> utils/trajectory.py:104-151) on the device: consecutive samples of
  * every trajectory of the reset table in observation layout. d_states / d_next_states fp32 [locosim_dataset_rows, obs_dim],
  * d_last fp32 [locosim_dataset_rows] (may be NULL); absorbing is all zero in the reference and is not materialised. */

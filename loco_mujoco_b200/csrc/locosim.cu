@@ -91,6 +91,7 @@ __global__ void reset_kernel(int ms, DevTask t, EngineState st, const uint8_t* m
     st.ws[(size_t)env * nv + i] = 0;
   }
   for (int k = lane; k < t.n_goal; k += 32) st.goal[(size_t)env * 4 + k] = row[2 * nv + k];
+  zero_applied(ms, env);
   if (obs) {
     for (int k = lane; k < t.obs_dim; k += 32) {
       int idx = t.obs_src_idx[k], ty = t.obs_src_type[k];
@@ -213,6 +214,7 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
   const int nv = m.nv, nu = m.nu, D = t.obs_dim;
   if (lane == 0) {
     e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
+    e.env = env;
     if (stage_bytes > 0) {
       const unsigned char* sm = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
       e.pk_tab = reinterpret_cast<const int*>(sm);
@@ -410,6 +412,7 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
   const int nv = m.nv, nu = m.nu, D = t.obs_dim;
   if (lane == 0) {
     e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
+    e.env = env;
     if (stage_bytes > 0) {
       const unsigned char* sm = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
       e.pk_tab = reinterpret_cast<const int*>(sm);
@@ -760,6 +763,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
   EnvS<C>& e = reinterpret_cast<EnvS<C>*>(smem_raw)[warp];
   const DevModel& m = c_models[ms];
   const int nv = m.nv, nu = m.nu, D = t.obs_dim;
+  e.env = env;     // (every lane: a predicated store costs the persistent kernel a spill)
   if (lane == 0) {
     e.prm = st.pool + (size_t)__ldcg(&st.dr_row[env]) * m.pool_P;
     if (stage_bytes > 0) {
@@ -1078,6 +1082,7 @@ struct locosim_handle {
   HostModel hm;
   HostTask ht;
   DevModel dm;
+  DevApplied applied = {nullptr, nullptr};
   DevTask dt;
   SolverOpts so;
   EngineState st;
@@ -1352,7 +1357,8 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
   bind_model(h->dm, h->hm, h->d_mints, h->d_mreals);
   for (int k = 0; k < LS_MAX_SLOTS && h->slot < 0; k++) if (!g_slot_used[k]) { h->slot = k; g_slot_used[k] = true; }
   if (h->slot < 0) { locosim_destroy(h); g_create_error = "too many live locosim handles (max 16 per process)"; return 1; }
-  if (cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess) {
+  if (cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot) != cudaSuccess) {
     g_create_error = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); return 1;
   }
   bind_task(h->dt, h->ht, h->hm.nu, h->d_tints, h->d_treals);
@@ -1420,6 +1426,15 @@ int locosim_get_cursor(locosim_t* h, int32_t* d_out, void* stream) {
 int locosim_set_time_limit(locosim_t* h, int max_episode_steps, int end_of_trajectory) {
   if (max_episode_steps < 0 || end_of_trajectory < 0) { h->err = "bad time limit (negative)"; return 1; }
   h->st.max_episode_steps = max_episode_steps; h->st.end_of_trajectory = end_of_trajectory ? 1 : 0;
+  return 0;
+}
+int locosim_nbody(const locosim_t* h) { return h->hm.nb; }
+int locosim_set_applied_forces(locosim_t* h, float* d_xfrc, float* d_qfrc) {
+  CK(cudaSetDevice(h->device));
+  h->applied.xfrc = d_xfrc; h->applied.qfrc = d_qfrc;
+  // (the kernels read the pointers from the handle's __constant__ slot, in both translation units)
+  CK(cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot));
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   return 0;
 }
 int locosim_get_episode_stats(locosim_t* h, int32_t* d_len, float* d_ret, int32_t* d_last_len, float* d_last_ret, void* stream) {

@@ -39,6 +39,7 @@ extern "C" {
 int locosim_configs31_sync_model(Handle31* h) {
   using namespace locosim31;
   CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
+  CK(cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot));
   return 0;
 }
 

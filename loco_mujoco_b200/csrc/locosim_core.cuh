@@ -36,6 +36,7 @@ struct alignas(16) float4 { float x, y, z, w; };
 #define LS_CLZ(x) __builtin_clz((unsigned)(x))
 #define BLOCK_ANY(flag, pred) (pred)
 #define BLOCK_SYNC(flag) ((void)0)
+#define LS_LDG(p) (*(p))
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 #else
 #define LS_DEV __device__ __forceinline__
@@ -48,6 +49,7 @@ static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 #define LS_LANE ((int)(threadIdx.x & 31))
 #define LS_FFS(x) __ffs((int)(x))
 #define LS_CLZ(x) __clz((int)(x))
+#define LS_LDG(p) __ldg(p)           // read-only path (caller-owned inputs that no warp writes before its last read)
 // OR-reduction that doubles as a barrier: keeps warps in the same solver iteration (flag = 0: plain predicate).
 // flag = number of consecutive warps that iterate in lock-step (a GROUP): flag >= warps per block -> the whole block
 // (__syncthreads_or); smaller groups use one named barrier each (barrier.red with a thread count), so a group only waits
@@ -115,6 +117,13 @@ struct DevModel {
       po_body_inertia, po_body_ipos, po_body_iquat, po_geom_friction, po_geom_invweight0, po_meaninertia, po_user, pool_P;
 };
 
+// applied forces of a handle (locosim_set_applied_forces): caller-owned [N, nb, 6] body wrenches (force, torque; world frame,
+// at the body's CoM) and [N, nv] generalised forces, row EnvS::env; NULL = none. The engine zeroes the rows of an env it resets.
+struct DevApplied {
+  float* xfrc;
+  float* qfrc;
+};
+
 struct DevTask {
   int obs_dim, n_done, reward_type, n_substeps, n_traj, traj_len, n_goal, recenter0, recenter1, ri[4], use_absorbing;
   int n_grf;                      // foot-force groups (use_foot_forces), 0 = off
@@ -131,9 +140,11 @@ struct DevTask {
 #define LS_MAX_SLOTS 16
 #ifdef LS_EMULATE
 static DevModel c_models[LS_MAX_SLOTS];
+static DevApplied c_applied[LS_MAX_SLOTS];
 static int c_debug = 0;
 #else
 __constant__ DevModel c_models[LS_MAX_SLOTS];
+__constant__ DevApplied c_applied[LS_MAX_SLOTS];   // (a table of its own: DevModel's layout, and the code reading it, stay as they are)
 __constant__ int c_debug;      // diagnostic switches (LOCOSIM_DEBUG): 1 skip MPR, 2 skip the OBB filter, 4 drop convex pairs,
                                // 8 count MPR runs / support calls (locosim_debug_counters), 16 no separating-direction cache
 __device__ unsigned long long g_dbg[8];      // (LOCOSIM_DEBUG & 8) MPR statistics: calls, support pairs, hits, cap exits
@@ -213,6 +224,8 @@ struct alignas(16) EnvS {
       unsigned char r_state[MAXEFC];
     };
   };
+  int env;                           // row of this env in the applied-force buffers (c_applied[ms]);
+                                     // sits in the alignment gap in front of J: sizeof(EnvS) is the same with and without it
   alignas(16) float J[MAXROW][JS];   // contact Jacobian rows, zero padded to a float4 multiple
 #ifdef LS_EMULATE
   float Y[6][NV];
@@ -1863,7 +1876,9 @@ LS_FN void smooth_forces(const int ms, EnvS<C>& e) {
   }
   SYNC();
   // (B) per body: cvel, cacc (gravity enters as the world's upward acceleration), f = I cacc + cvel x* (I cvel)
-  //     -> crb[b][0..5] (the composite inertias are dead once M is assembled)
+  //     -> crb[b][0..5] (the composite inertias are dead once M is assembled); minus the applied wrench, moved from the
+  //     body's CoM to the frame's origin e.com (mj_xfrcAccumulate: pass (C) turns it into J^T wrench in qfrc_smooth)
+  const float* __restrict__ xfrc = c_applied[ms].xfrc;
   PAR_FOR(b, m.nb) {
     float* f = e.crb[b];
     if (b == 0) { for (int k = 0; k < 6; k++) f[k] = 0; continue; }
@@ -1880,9 +1895,18 @@ LS_FN void smooth_forces(const int ms, EnvS<C>& e) {
     mulInertVec(t2, e.cinert[b], cvel);
     crossForce(t3, cvel, t2);
     for (int k = 0; k < 6; k++) f[k] = t1[k] + t3[k];
+    if (xfrc) {
+      const float* w = xfrc + ((size_t)e.env * m.nb + b) * 6;
+      const float F[3] = {LS_LDG(w), LS_LDG(w + 1), LS_LDG(w + 2)};
+      const float r[3] = {e.xipos[b][0] - e.com[0], e.xipos[b][1] - e.com[1], e.xipos[b][2] - e.com[2]};
+      float rxF[3];
+      cross3(rxF, r, F);
+      for (int k = 0; k < 3; k++) { f[k] -= LS_LDG(w + 3 + k) + rxF[k]; f[3 + k] -= F[k]; }
+    }
   }
   SYNC();
-  // (C) bias force of dof j = cdof_j . (sum of f over the bodies below j);  qfrc_smooth = passive - bias + actuator
+  // (C) bias force of dof j = cdof_j . (sum of f over the bodies below j);  qfrc_smooth = passive - bias + applied + actuator
+  const float* __restrict__ qfrc = c_applied[ms].qfrc;
   PAR_FOR(j, nv) {
     float F[6] = {0, 0, 0, 0, 0, 0};
     NOUNROLL for (int b = 1; b < m.nb; b++) {
@@ -1892,7 +1916,7 @@ LS_FN void smooth_forces(const int ms, EnvS<C>& e) {
     float bias = 0;
     for (int c = 0; c < 6; c++) bias += e.cdof[j][c] * F[c];
     float passive = -PRM(jnt_stiffness)[j] * (e.qpos[j] - m.qpos_spring[j]) - PRM(dof_damping)[j] * e.qvel[j];
-    e.qfrc_smooth[j] = passive - bias;
+    e.qfrc_smooth[j] = qfrc ? passive - bias + LS_LDG(qfrc + (size_t)e.env * nv + j) : passive - bias;
   }
   SYNC();
   PAR_FOR(i, m.nu) {
@@ -2777,6 +2801,14 @@ LS_DEV float reset_value(const DevTask& t, const float* row, int nv, int kind, i
   return v;
 }
 
+// every reset of an env zeroes its rows of the applied-force buffers (mj_resetData); a whole-warp call
+LS_DEV void zero_applied(const int ms, const int env) {
+  const DevModel& m = c_models[ms];
+  const DevApplied& ap = c_applied[ms];
+  if (ap.xfrc) PAR_FOR(k, 6 * m.nb) ap.xfrc[(size_t)env * 6 * m.nb + k] = 0.0f;
+  if (ap.qfrc) PAR_FOR(k, m.nv) ap.qfrc[(size_t)env * m.nv + k] = 0.0f;
+}
+
 template <class C>
 LS_FN void reset_env(const int ms, const DevTask& t, EnvS<C>& e, int traj_no, int step_no, float angle) {
   const DevModel& m = c_models[ms];
@@ -2789,5 +2821,6 @@ LS_FN void reset_env(const int ms, const DevTask& t, EnvS<C>& e, int traj_no, in
   }
   PAR_FOR(k, t.n_goal) e.goal[k] = row[2 * nv + k];
   PAR_FOR(k, 3 * LS_MAX_GRF) e.grf[k] = 0;     // mean_grf is reset with the episode (reset observation: zeros)
+  zero_applied(ms, e.env);
   SYNC();
 }

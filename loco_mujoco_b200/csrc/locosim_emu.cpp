@@ -11,6 +11,7 @@
 struct EmuBase {
   HostModel hm;
   DevModel m;
+  DevApplied ap = {nullptr, nullptr};
   SolverOpts so;
   std::vector<int> grf_group; int n_grf = 0;
   virtual ~EmuBase() {}
@@ -35,12 +36,12 @@ struct EmuT : EmuBase {
   }
   void step(const double* ctrl, int nsub) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
-    c_models[0] = m;
+    c_models[0] = m; c_applied[0] = ap;
     physics_substeps(0, e, so, nsub, grf_group.data(), n_grf);
   }
   void fwd(const double* ctrl) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
-    c_models[0] = m;
+    c_models[0] = m; c_applied[0] = ap;
     forward(0, e, so);
   }
   void get(double* q, double* v, double* qacc, double* ws) override {
@@ -73,7 +74,7 @@ struct EmuT : EmuBase {
     for (int i = 0; i < m.nv; i++) { e.qpos[i] = keep->qpos[i]; e.qvel[i] = keep->qvel[i]; e.qacc_ws[i] = keep->qacc_ws[i]; e.qacc[i] = 0; }
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = keep->ctrl[i];
     for (int k = 0; k < 4; k++) e.goal[k] = keep->goal[k];
-    e.prm = keep->prm; e.pk_tab = keep->pk_tab;
+    e.prm = keep->prm; e.pk_tab = keep->pk_tab; e.env = keep->env;
     init_workspace(0, e);
     e.iter_sum = keep->iter_sum; e.mpr_calls = keep->mpr_calls; e.sep_next = keep->sep_next;
     for (int k = 0; k < EnvS<C>::NSEP; k++) {
@@ -124,6 +125,9 @@ void emu_get_state(EmuBase* s, double* qpos, double* qvel) { s->get(qpos, qvel, 
 void emu_get_qacc(EmuBase* s, double* qacc) { s->get(nullptr, nullptr, qacc, nullptr); }
 void emu_get_ws(EmuBase* s, double* w) { s->get(nullptr, nullptr, nullptr, w); }
 void emu_set_ws(EmuBase* s, const double* w) { s->set_ws(w); }
+// applied forces of the emulated env (row 0 of the engine's layout: xfrc fp32 [nb, 6], qfrc fp32 [nv]; either may be NULL),
+// read by every later emu_step / emu_forward from the caller's memory
+void emu_set_applied(EmuBase* s, float* xfrc, float* qfrc) { s->ap.xfrc = xfrc; s->ap.qfrc = qfrc; }
 long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, 0}; return v[k]; }
 long emu_ls_evals() { return g_ls_evals; }
 long emu_ls_searches() { return g_ls_searches; }

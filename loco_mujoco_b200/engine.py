@@ -78,6 +78,10 @@ def load_library():
     lib.locosim_set_time_limit.argtypes = [vp, ip, ip]
     lib.locosim_get_episode_stats.restype = ip
     lib.locosim_get_episode_stats.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.locosim_nbody.restype = ip
+    lib.locosim_nbody.argtypes = [vp]
+    lib.locosim_set_applied_forces.restype = ip
+    lib.locosim_set_applied_forces.argtypes = [vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -89,7 +93,7 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_kernels_per_step", "locosim_reset_rows", "locosim_set_goal", "locosim_measure_fp32_peak",
                     "locosim_set_reset_rotation", "locosim_get_cursor", "locosim_dataset_rows", "locosim_create_dataset",
                     "locosim_debug_counters", "locosim_set_timeline", "locosim_set_time_limit",
-                    "locosim_get_episode_stats"]
+                    "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces"]
 
 # bits of the done byte of a step (include/locosim.h)
 DONE_ABSORBING, DONE_TRUNCATED = 1, 2
@@ -158,6 +162,8 @@ class CudaEngine:
         self.obs_dim = self.lib.locosim_obs_dim(h)
         self.action_dim = self.lib.locosim_action_dim(h)
         self.nq = self.lib.locosim_nq(h)
+        self.nbody = self.lib.locosim_nbody(h)
+        self._applied = (None, None)      # the registered applied-force tensors (kept alive while registered)
         # obs / reward / done of a step live in ONE device allocation (three views), so that a consumer on the host can
         # fetch the whole step result with a single D2H copy of `packed_out`
         N, D = int(n_envs), self.obs_dim
@@ -249,6 +255,22 @@ class CudaEngine:
         """Time limit of include/locosim.h: truncate an episode at `max_episode_steps` control steps (0 = no limit) and / or
         where its trajectory cursor reaches the last mocap sample. Reported as bit 1 of `done`; takes effect from the next step."""
         self._check(self.lib.locosim_set_time_limit(self.h, int(max_episode_steps), int(bool(end_of_trajectory))))
+
+    def set_applied_forces(self, xfrc=None, qfrc=None):
+        """Register the applied forces of include/locosim.h (MuJoCo's xfrc_applied / qfrc_applied): `xfrc` float32 cuda
+        [n_envs, nbody, 6] (force then torque, world frame, at each body's centre of mass; body 0 ignored), `qfrc` float32
+        cuda [n_envs, nq]; either None. The engine reads the tensors in every later step, zeroes the rows of every env it
+        resets, and keeps a reference to them. None, None turns the feature off. Register outside of CUDA-graph capture."""
+        t = self.torch
+        for x, shape, name in ((xfrc, (self.n_envs, self.nbody, 6), "xfrc"), (qfrc, (self.n_envs, self.nq), "qfrc")):
+            if x is None:
+                continue
+            if x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
+                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+            if tuple(x.shape) != shape:
+                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+        self._check(self.lib.locosim_set_applied_forces(self.h, _ptr(xfrc), _ptr(qfrc)))
+        self._applied = (xfrc, qfrc)
 
     def episode_stats(self):
         """(length int32, return float32, last_length, last_return), each [n_envs]: the running episode's control steps and

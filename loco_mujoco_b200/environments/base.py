@@ -235,6 +235,9 @@ class LocoEnv:
         # step() reports `info["truncated"]`, and batched envs reset truncated episodes in the same step like fallen ones.
         self._max_episode_steps = resolve_time_limit(time_limit, horizon)
         self._truncate_at_trajectory_end = bool(truncate_at_trajectory_end)
+        # applied forces (xfrc_applied / qfrc_applied below): allocated and registered with the engine on first access
+        self._xfrc_applied = None
+        self._qfrc_applied = None
         self._engine = None
         self._obs = None
 
@@ -425,7 +428,45 @@ class LocoEnv:
                 self._engine.set_param_pool(self.model_pool())
             if self.time_limited:
                 self._engine.set_time_limit(self._max_episode_steps, self._truncate_at_trajectory_end)
+            if self._xfrc_applied is not None or self._qfrc_applied is not None:
+                self._engine.set_applied_forces(self._xfrc_applied, self._qfrc_applied)
         return self._engine
+
+    # ---------------------------------------------------------------------------------------------------
+    # applied forces (MuJoCo's mjData.xfrc_applied / qfrc_applied, include/locosim.h locosim_set_applied_forces)
+    # ---------------------------------------------------------------------------------------------------
+    def body_index(self, name):
+        """Row of body `name` in `xfrc_applied` (an index of the compiled model). ValueError for an unknown name and for a
+        body that fuse_static merged into its parent; the message then names the parent."""
+        return self._model.body_index(name)
+
+    @property
+    def xfrc_applied(self):
+        """float32 torch tensor [num_envs, nbody, 6] on the env's device: per body a force (3) then a torque (3) in world
+        coordinates, applied at the body's centre of mass in every dynamics evaluation of every later step (row 0, the world,
+        is ignored). Write into it in place (also between replays of a captured CUDA graph); it keeps its values until you
+        change them, except that every reset of an env (reset(), the auto-reset of a fallen or truncated env) zeroes that
+        env's rows. Allocated zeroed and registered with the engine on first access: an env that never touches it runs the
+        step without applied forces."""
+        if self._xfrc_applied is None:
+            self._xfrc_applied = self._new_applied((self.num_envs, self._model.nbody, 6))
+        return self._xfrc_applied
+
+    @property
+    def qfrc_applied(self):
+        """float32 torch tensor [num_envs, nq] of generalised forces added to the joint forces in every dynamics
+        evaluation (MuJoCo's qfrc_applied). Same life cycle as `xfrc_applied`."""
+        if self._qfrc_applied is None:
+            self._qfrc_applied = self._new_applied((self.num_envs, self._model.nv))
+        return self._qfrc_applied
+
+    def _new_applied(self, shape):
+        import torch
+        eng = self._get_engine()
+        t = torch.zeros(shape, dtype=torch.float32, device=eng.device)
+        x, q = (t, self._qfrc_applied) if len(shape) == 3 else (self._xfrc_applied, t)
+        eng.set_applied_forces(x, q)
+        return t
 
     # ---------------------------------------------------------------------------------------------------
     # the hot path

@@ -291,6 +291,15 @@ class HumanoidTorque4AgesAll:
     def dt(self):
         return self.subs[0].dt
 
+    # ---- applied forces: the four humanoids differ in their bodies and the envs are interleaved over four engines ----
+    def _no_applied_forces(self, *args):
+        raise NotImplementedError("applied forces (xfrc_applied / qfrc_applied / body_index) are not available for "
+                                  "HumanoidTorque4Ages mode 'all': use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
+
+    xfrc_applied = property(_no_applied_forces)
+    qfrc_applied = property(_no_applied_forces)
+    body_index = _no_applied_forces
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch

@@ -279,6 +279,17 @@ class Model:
     def body_id(self, name):
         return self.body_names.index(name)
 
+    def body_index(self, name):
+        """Index of body `name` in the compiled model (the row of LocoEnv.xfrc_applied). ValueError for an unknown name and
+        for a body that fuse_static merged into its parent (the message names the body it now belongs to)."""
+        if name in self.body_names:
+            return self.body_names.index(name)
+        fused = getattr(self, "fused_bodies", {})
+        if name in fused:
+            raise ValueError("body %r has no joint and was fused into %r (fuse_static=True): apply the force to %r"
+                             % (name, fused[name], fused[name]))
+        raise ValueError("unknown body %r (bodies of the compiled model: %s)" % (name, ", ".join(self.body_names)))
+
 
 def _orientation(attrs, comp):
     if "quat" in attrs:
@@ -992,6 +1003,15 @@ def fuse_static_bodies(m):
                 parent[c2] = p
         alive[b] = False
     keep = np.nonzero(alive)[0]
+    # name of every fused body -> name of the body it now belongs to (parent[b] is b's parent when b was fused)
+    fused = {}
+    for b in range(1, nb):
+        if not alive[b]:
+            p = parent[b]
+            while not alive[p]:
+                p = parent[p]
+            fused[m.body_names[b]] = m.body_names[p]
+    m.fused_bodies = fused
     remap = -np.ones(nb, dtype=np.int64)
     remap[keep] = np.arange(len(keep))
     inertia, iquat = np.zeros((len(keep), 3)), np.zeros((len(keep), 4))

@@ -68,6 +68,10 @@ def to_npz_dict(m):
         d["scalar_" + s] = np.asarray(getattr(m, s))
     for n in NAME_LISTS:
         d["names_" + n] = np.array(getattr(m, n), dtype=object).astype(str)
+    fused = getattr(m, "fused_bodies", None)
+    if fused:      # (optional: which body each static body was fused into, for Model.body_index's message)
+        d["names_fused_from"] = np.array(list(fused), dtype=object).astype(str)
+        d["names_fused_into"] = np.array(list(fused.values()), dtype=object).astype(str)
     return d
 
 
@@ -81,4 +85,6 @@ def from_npz_dict(d):
         setattr(m, s, v.item())
     for n in NAME_LISTS:
         setattr(m, n, [str(x) for x in d["names_" + n]])
+    if "names_fused_from" in d:
+        m.fused_bodies = {str(a): str(b) for a, b in zip(d["names_fused_from"], d["names_fused_into"])}
     return m
