@@ -132,6 +132,36 @@ int locosim_nbody(const locosim_t* h);
  * it is replayed. */
 int locosim_set_applied_forces(locosim_t* h, float* d_xfrc, float* d_qfrc);
 
+/* Body outputs, MuJoCo's per-body kinematics (what a loco-mujoco user reads from env._data: xpos, xquat, body velocities):
+ * caller-owned DEVICE buffers, each fp32 [n_envs, nbody, LS_BODY_DIM]. Per body (row) 13 values:
+ *   xpos (3)  world position of the body frame
+ *   xquat (4) orientation of the body frame, w x y z
+ *   angular velocity (3), then linear velocity (3) of the body-frame origin xpos, both in world coordinates: the result of
+ *             mj_objectVelocity(m, d, mjOBJ_XBODY, b, res, 0), in its order. The point is the body-frame origin, NOT the centre
+ *             of mass (xipos) that xfrc_applied acts at.
+ * Row 0 (the world) is (0,0,0, 1,0,0,0, 0,0,0, 0,0,0). Body indices are those of the compiled model, as for xfrc_applied.
+ * The values describe the state they are written for: mj_kinematics + mj_comPos + mj_comVel evaluated on that state's qpos /
+ * qvel, i.e. what mj_forward on that state gives. This differs from MuJoCo's mjData after mj_step, whose kinematic fields
+ * still describe the start of the last sub-step (after RK4: its last stage); here they describe the same state as the
+ * observation.
+ *   d_body:      written by every locosim_step for the state d_obs describes: for an env that ended, its terminal state
+ *                (before the auto-reset); for a non-finite env all zeros, as its observation.
+ *   d_next_body: always the state locosim_get_state returns: written by locosim_step after the auto-reset (rows of envs not
+ *                reset equal d_body bit for bit), by locosim_reset* for the masked envs and by locosim_set_state for every env.
+ * While either is registered, locosim_step enqueues one more kernel after the step (the rows of envs it resets are written
+ * by the step kernel before the reset, every other row from the stored state), and locosim_reset* / locosim_set_state one
+ * kernel each when d_next_body is registered. Either may be NULL; NULL, NULL = off = the state after locosim_create (nothing
+ * is written or launched then, and no other output changes by a bit; with buffers registered no other output changes by a
+ * bit either). Register outside of stream capture, like locosim_set_applied_forces.
+ * CUDA graphs: whether the extra kernel is part of a step is decided when the step is enqueued (or captured). A graph captured
+ * while something is registered writes, at each replay, into whatever non-NULL buffers are registered then (a later
+ * registration of other buffers is picked up; NULL, NULL makes its extra kernel write nothing). A graph captured while
+ * NOTHING was registered never writes d_next_body, nor d_body of envs it does not reset: after turning the feature on,
+ * capture the step again. (Each registration clears the engine's per-env reset marks, and under auto_reset the rows an
+ * eager or re-captured step writes never depend on what such a stale graph did.) */
+#define LS_BODY_DIM 13
+int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body);
+
 /* Replaces LocoEnv.create_dataset() (base.py:278-312 -> utils/trajectory.py:104-151) on the device: consecutive samples of
  * every trajectory of the reset table in observation layout. d_states / d_next_states fp32 [locosim_dataset_rows, obs_dim],
  * d_last fp32 [locosim_dataset_rows] (may be NULL); absorbing is all zero in the reference and is not materialised. */

@@ -1038,6 +1038,50 @@ __global__ void __launch_bounds__(512, 1) persist_kernel(int ms, DevTask t, Solv
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// Body-output kernel (locosim_set_body_outputs), one warp and one EnvS per block, from the engine's state (the env's
+// parameter-pool row as in the step kernels: masses and inertial frames differ per env under domain randomisation and carry
+// tasks). After a step (done = that step's done bytes, every env): d_next_body, and d_body of the envs the step did not
+// reset (the same state). The envs the step reset are those with a done byte under auto_reset, and those reset_env marked
+// (a non-finite env) without it; reset_env has written their d_body rows from the terminal state, which the stored state no
+// longer holds. After locosim_reset* (the envs of `mask`) and locosim_set_state (all, done = NULL): d_next_body.
+// Why the rows are not all written by the step kernels: their terminal rows must be (nothing else sees the terminal state),
+// and reset_env is a call those kernels already make; a body-output call of their own, in every epilogue, changes their
+// register allocation and stack frames, which the off path must not pay for. This kernel is enqueued only while buffers
+// are registered.
+// ----------------------------------------------------------------------------------------------------------
+template <class C>
+__global__ void __launch_bounds__(32) body_kernel(int ms, EngineState st, const uint8_t* __restrict__ mask,
+                                                  const uint8_t* __restrict__ done, int auto_reset) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int env = blockIdx.x, lane = threadIdx.x & 31;
+  if (mask && !mask[env]) return;
+  EnvS<C>& e = *reinterpret_cast<EnvS<C>*>(smem_raw);
+  const DevModel& m = c_models[ms];
+  const DevBodyOut bo = c_bodyout[ms];
+  const int nv = m.nv;
+  const size_t off = (size_t)env * m.nb * LS_BODY_DIM;
+  float* body = nullptr;
+  if (done && bo.body) {
+    // (under auto_reset the done byte alone decides: a mark left by a step that was not followed by this kernel cannot
+    // hide a row; every mark is cleared here)
+    const int mark = bo.reset_mark[env];
+    const bool was_reset = done[env] != 0 && (auto_reset || mark != 0);
+    __syncwarp();
+    if (!was_reset) body = bo.body + off;
+    if (lane == 0 && mark) bo.reset_mark[env] = 0;
+  }
+  float* next = bo.next_body ? bo.next_body + off : nullptr;
+  if (!body && !next) return;
+  if (lane == 0) e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
+  for (int i = lane; i < nv; i += 32) {
+    e.qpos[i] = st.qpos[(size_t)env * nv + i];
+    e.qvel[i] = st.qvel[(size_t)env * nv + i];
+  }
+  __syncwarp();
+  body_outputs(ms, e, body, next);
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // Regrouping: the warps of a block run the solver in lock-step, so a block is as slow as its hardest env. Solver effort
 // is strongly correlated from one control step to the next (lag-1 correlation of the per-step Newton iteration count
 // ~0.6), so before every step the envs are bucketed by the iteration count of their previous step (counting sort,
@@ -1083,6 +1127,7 @@ struct locosim_handle {
   HostTask ht;
   DevModel dm;
   DevApplied applied = {nullptr, nullptr};
+  DevBodyOut bodyout = {nullptr, nullptr, nullptr};
   DevTask dt;
   SolverOpts so;
   EngineState st;
@@ -1116,6 +1161,13 @@ static_assert(sizeof(EnvS<CfgPyrRK4>) * 14 <= 232448, "HumanoidTorque / Atlas: 1
 static_assert(sizeof(EnvS<CfgPyrEuler29>) * 9 <= 232448, "UnitreeG1: 9 envs per SM");
 
 template <class C>
+static int launch_body(locosim_handle* h, const uint8_t* mask, const uint8_t* done, int auto_reset, cudaStream_t s) {
+  static_assert(sizeof(EnvS<C>) <= 48 * 1024, "body_kernel: one EnvS per block within the default shared-memory limit");
+  body_kernel<C><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, mask, done, auto_reset);
+  CK(cudaGetLastError());
+  return 0;
+}
+template <class C>
 static int launch_step(locosim_handle* h, const float* a, float* o, float* r, uint8_t* d, float* no, int auto_reset,
                        cudaStream_t s) {
   int blocks = (h->n_envs + h->wpb - 1) / h->wpb;
@@ -1137,6 +1189,8 @@ static int launch_step(locosim_handle* h, const float* a, float* o, float* r, ui
                                                          h->split);
   }
   CK(cudaGetLastError());
+  // body outputs (only while registered): the rows the step kernel did not write
+  if (h->bodyout.body || h->bodyout.next_body) return launch_body<C>(h, nullptr, d, auto_reset, s);
   return 0;
 }
 template <class C>
@@ -1299,6 +1353,21 @@ extern "C" int locosim_configs31_setup(locosim_handle* h) __attribute__((weak));
 extern "C" int locosim_configs31_step(locosim_handle* h, const float* a, float* o, float* r, uint8_t* d, float* no,
                                       int auto_reset, cudaStream_t s) __attribute__((weak));
 extern "C" int locosim_configs31_sync_model(locosim_handle* h) __attribute__((weak));
+extern "C" int locosim_configs31_body(locosim_handle* h, const uint8_t* mask, cudaStream_t s) __attribute__((weak));
+
+// d_next_body rows of the envs of `mask` (NULL = all), when registered: after locosim_reset* and locosim_set_state
+static int next_body_rows(locosim_handle* h, const uint8_t* mask, cudaStream_t s) {
+  if (!h->bodyout.next_body) return 0;
+  switch (h->cfg) {
+    case 0: return launch_body<CfgEllEuler>(h, mask, nullptr, 0, s);
+    case 1: return launch_body<CfgPyrEuler>(h, mask, nullptr, 0, s);
+    case 3: return launch_body<CfgPyrEuler29>(h, mask, nullptr, 0, s);
+    case 4:
+    case 5: return locosim_configs31_body(h, mask, s);
+    default: return launch_body<CfgPyrRK4>(h, mask, nullptr, 0, s);
+  }
+}
+
 
 extern "C" {
 
@@ -1358,7 +1427,8 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
   for (int k = 0; k < LS_MAX_SLOTS && h->slot < 0; k++) if (!g_slot_used[k]) { h->slot = k; g_slot_used[k] = true; }
   if (h->slot < 0) { locosim_destroy(h); g_create_error = "too many live locosim handles (max 16 per process)"; return 1; }
   if (cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess ||
-      cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot) != cudaSuccess) {
+      cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot) != cudaSuccess) {
     g_create_error = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); return 1;
   }
   bind_task(h->dt, h->ht, h->hm.nu, h->d_tints, h->d_treals);
@@ -1394,6 +1464,7 @@ void locosim_destroy(locosim_t* h) {
   cudaFree(h->d_stage);
   cudaFree(h->split.carry); cudaFree(h->split.bcount); cudaFree(h->split.benv); cudaFree(h->split.seq);
   cudaFree(h->pq.carry); cudaFree(h->pq.cnt); cudaFree(h->pq.tot); cudaFree(h->pq.benv); cudaFree(h->pq.seq);
+  cudaFree(h->bodyout.reset_mark);
   delete h;
 }
 
@@ -1416,7 +1487,7 @@ int locosim_reset_rows(locosim_t* h, const uint8_t* d_mask, const int32_t* d_tra
                                                              h->n_envs, h->seed, h->env_off);
   h->st.rot_angle = nullptr;        // pinned rotation angles apply to one reset call
   CK(cudaGetLastError());
-  return 0;
+  return next_body_rows(h, d_mask, (cudaStream_t)stream);
 }
 int locosim_set_reset_rotation(locosim_t* h, const float* d_angle) { h->st.rot_angle = d_angle; return 0; }
 int locosim_get_cursor(locosim_t* h, int32_t* d_out, void* stream) {
@@ -1434,6 +1505,18 @@ int locosim_set_applied_forces(locosim_t* h, float* d_xfrc, float* d_qfrc) {
   h->applied.xfrc = d_xfrc; h->applied.qfrc = d_qfrc;
   // (the kernels read the pointers from the handle's __constant__ slot, in both translation units)
   CK(cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot));
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  return 0;
+}
+int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body) {
+  CK(cudaSetDevice(h->device));
+  if (d_body && !h->bodyout.reset_mark) CK(cudaMalloc((void**)&h->bodyout.reset_mark, (size_t)h->n_envs * 4));
+  // one flag per env: set by the step kernel's reset_env where it wrote d_body, cleared by the body_kernel after the step;
+  // cleared on every registration, so that no mark from earlier steps survives into the new buffers
+  if (h->bodyout.reset_mark) CK(cudaMemset(h->bodyout.reset_mark, 0, (size_t)h->n_envs * 4));
+  h->bodyout.body = d_body; h->bodyout.next_body = d_next_body;
+  // (a __constant__ table of its own in both translation units, like the applied forces)
+  CK(cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot));
   if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   return 0;
 }
@@ -1510,7 +1593,7 @@ int locosim_set_state(locosim_t* h, const float* q, const float* v, const float*
   if (v) CK(cudaMemcpyAsync(h->st.qvel, v, bytes, cudaMemcpyDeviceToDevice, s));
   if (w) CK(cudaMemcpyAsync(h->st.ws, w, bytes, cudaMemcpyDeviceToDevice, s));
   else CK(cudaMemsetAsync(h->st.ws, 0, bytes, s));
-  return 0;
+  return next_body_rows(h, nullptr, s);
 }
 int locosim_set_goal(locosim_t* h, const float* g, void* stream) {
   if (!g) { h->err = "null buffer"; return 1; }
@@ -1565,9 +1648,10 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
 
 int locosim_kernels_per_step(const locosim_t* h) {
   const int nsub = h->dt.n_substeps;
-  if (h->persist) return 1;
-  if (h->resort < nsub) return (nsub + h->resort - 1) / h->resort;
-  return h->regroup ? 2 : 1;
+  const int body = h->bodyout.body || h->bodyout.next_body ? 1 : 0;    // (body_kernel, while body outputs are registered)
+  if (h->persist) return 1 + body;
+  if (h->resort < nsub) return (nsub + h->resort - 1) / h->resort + body;
+  return (h->regroup ? 2 : 1) + body;
 }
 int locosim_set_timeline(locosim_t* h, long long* d_records, int capacity) {
   if (!h->persist) { h->err = "the timeline is recorded by the persistent sub-step kernel only"; return 1; }

@@ -40,6 +40,7 @@ int locosim_configs31_sync_model(Handle31* h) {
   using namespace locosim31;
   CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
   CK(cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot));
+  CK(cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot));
   return 0;
 }
 
@@ -59,6 +60,15 @@ int locosim_configs31_step(Handle31* h, const float* a, float* o, float* r, uint
   switch (h->cfg) {
     case 4: return launch_step<CfgPyrRK4_31>(h, a, o, r, d, no, auto_reset, s);
     case 5: return launch_step<CfgPyrEuler31>(h, a, o, r, d, no, auto_reset, s);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
+int locosim_configs31_body(Handle31* h, const uint8_t* mask, cudaStream_t s) {
+  using namespace locosim31;
+  switch (h->cfg) {
+    case 4: return launch_body<CfgPyrRK4_31>(h, mask, nullptr, 0, s);
+    case 5: return launch_body<CfgPyrEuler31>(h, mask, nullptr, 0, s);
     default: h->err = "not a 31-dof configuration"; return 1;
   }
 }

@@ -17,6 +17,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "../../include/locosim.h"            // (LS_BODY_DIM)
 #include "../../include/locosim_modelpack.h"
 #include "../../include/locosim_task.h"
 
@@ -124,6 +125,15 @@ struct DevApplied {
   float* qfrc;
 };
 
+// body outputs of a handle (locosim_set_body_outputs): caller-owned [N, nb, LS_BODY_DIM] rows (xpos, xquat, angular and linear
+// velocity of the body-frame origin, world frame) of the returned state (`body`) and of the state to act on next
+// (`next_body`); NULL = not written. reset_mark [N] (engine-owned): set where a step's reset_env wrote the env's `body` rows.
+struct DevBodyOut {
+  float* body;
+  float* next_body;
+  int* reset_mark;
+};
+
 struct DevTask {
   int obs_dim, n_done, reward_type, n_substeps, n_traj, traj_len, n_goal, recenter0, recenter1, ri[4], use_absorbing;
   int n_grf;                      // foot-force groups (use_foot_forces), 0 = off
@@ -141,10 +151,12 @@ struct DevTask {
 #ifdef LS_EMULATE
 static DevModel c_models[LS_MAX_SLOTS];
 static DevApplied c_applied[LS_MAX_SLOTS];
+static DevBodyOut c_bodyout[LS_MAX_SLOTS];
 static int c_debug = 0;
 #else
 __constant__ DevModel c_models[LS_MAX_SLOTS];
 __constant__ DevApplied c_applied[LS_MAX_SLOTS];   // (a table of its own: DevModel's layout, and the code reading it, stay as they are)
+__constant__ DevBodyOut c_bodyout[LS_MAX_SLOTS];  // (likewise)
 __constant__ int c_debug;      // diagnostic switches (LOCOSIM_DEBUG): 1 skip MPR, 2 skip the OBB filter, 4 drop convex pairs,
                                // 8 count MPR runs / support calls (locosim_debug_counters), 16 no separating-direction cache
 __device__ unsigned long long g_dbg[8];      // (LOCOSIM_DEBUG & 8) MPR statistics: calls, support pairs, hits, cap exits
@@ -2809,11 +2821,67 @@ LS_DEV void zero_applied(const int ms, const int env) {
   if (ap.qfrc) PAR_FOR(k, m.nv) ap.qfrc[(size_t)env * m.nv + k] = 0.0f;
 }
 
+// ----------------------------------------------------------------------------------------------------------
+// body outputs (locosim_set_body_outputs): mj_kinematics + mj_comPos + mj_comVel on the env's current qpos / qvel, then per
+// body xpos, xquat and the velocity of the body-frame origin (mj_objectVelocity, mjOBJ_XBODY, world frame: angular, linear)
+// ----------------------------------------------------------------------------------------------------------
+// A whole-warp call. It rewrites the kinematics (xpos, xquat, xmat, gxpos, com, cdof) and the smooth-dynamics scratch of the
+// union; every forward() recomputes all of them before reading them, and nothing a sub-step launch carries to the next one
+// (SplitState / PersistQueue carry record: counters, separating directions, foot forces) lives there. LS_BODY_DIM floats
+// per body go to dst and to dst2 (either may be NULL).
+template <class C>
+LS_FN void body_outputs(const int ms, EnvS<C>& e, float* dst, float* dst2) {
+  const DevModel& m = c_models[ms];
+  kinematics(ms, e);
+  com_pos(ms, e);
+  PAR_FOR(b, m.nb) {
+    // spatial velocity at e.com (mj_comVel): sum of cdof_d qvel_d over the dofs on the path root..b
+    float v[6] = {0, 0, 0, 0, 0, 0};
+    unsigned mask = (unsigned)m.body_dofmask[b];
+    while (mask) {
+      const int d = LS_FFS(mask) - 1;
+      mask &= mask - 1u;
+      const float qd = e.qvel[d];
+      for (int c = 0; c < 6; c++) v[c] += e.cdof[d][c] * qd;
+    }
+    // linear part moved from e.com to xpos: v + w x (xpos - com)
+    const float r[3] = {e.xpos[b][0] - e.com[0], e.xpos[b][1] - e.com[1], e.xpos[b][2] - e.com[2]};
+    float wr[3];
+    cross3(wr, v, r);
+    float o[LS_BODY_DIM] = {e.xpos[b][0], e.xpos[b][1], e.xpos[b][2], e.xquat[b][0], e.xquat[b][1], e.xquat[b][2],
+                            e.xquat[b][3], v[0], v[1], v[2], v[3] + wr[0], v[4] + wr[1], v[5] + wr[2]};
+    if (b == 0) for (int k = 7; k < LS_BODY_DIM; k++) o[k] = 0.0f;      // (the world: exact zeros, not 0 * x)
+    if (dst) for (int k = 0; k < LS_BODY_DIM; k++) dst[b * LS_BODY_DIM + k] = o[k];
+    if (dst2) for (int k = 0; k < LS_BODY_DIM; k++) dst2[b * LS_BODY_DIM + k] = o[k];
+  }
+  SYNC();
+}
+
+// d_body rows of an env the step kernel is about to reset (whole warp, from reset_env): its returned state exists only until
+// reset_env overwrites it. Zeros for a non-finite env (the epilogue's test; such an env is always reset). The env is marked,
+// and body_kernel, which writes every other row from the stored state after the step, leaves these rows alone.
+template <class C>
+LS_DEV void body_rows_terminal(const int ms, EnvS<C>& e, const int env) {
+  const DevBodyOut bo = c_bodyout[ms];
+  if (!bo.body) return;
+  const DevModel& m = c_models[ms];
+  bool bad = false;
+  PAR_FOR(i, m.nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+#ifndef LS_EMULATE
+  bad = __any_sync(0xffffffffu, bad);
+#endif
+  float* body = bo.body + (size_t)env * m.nb * LS_BODY_DIM;
+  if (bad) PAR_FOR(k, m.nb * LS_BODY_DIM) body[k] = 0.0f;
+  else body_outputs(ms, e, body, (float*)nullptr);
+  LANE0 bo.reset_mark[env] = 1;
+}
+
 template <class C>
 LS_FN void reset_env(const int ms, const DevTask& t, EnvS<C>& e, int traj_no, int step_no, float angle) {
   const DevModel& m = c_models[ms];
   const int nv = m.nv, ncol = 2 * nv + t.n_goal;
   const float* row = t.table + ((size_t)traj_no * t.traj_len + step_no) * ncol;
+  body_rows_terminal(ms, e, e.env);            // d_body of the terminal state, before it is overwritten
   PAR_FOR(i, nv) {
     e.qpos[i] = reset_value(t, row, nv, LS_OBS_QPOS, i, angle);
     e.qvel[i] = reset_value(t, row, nv, LS_OBS_QVEL, i, angle);

@@ -26,6 +26,7 @@ struct EmuBase {
   virtual void grf(double* o, int clear) = 0;
   virtual void frames(double* gx, double* bx) = 0;
   virtual void poison() = 0;
+  virtual void body(float* out) = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -84,6 +85,7 @@ struct EmuT : EmuBase {
     for (int k = 0; k < 3 * LS_MAX_GRF; k++) e.grf[k] = keep->grf[k];
     delete keep;
   }
+  void body(float* out) override { c_models[0] = m; body_outputs(0, e, out, (float*)nullptr); }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
 
@@ -128,6 +130,8 @@ void emu_set_ws(EmuBase* s, const double* w) { s->set_ws(w); }
 // applied forces of the emulated env (row 0 of the engine's layout: xfrc fp32 [nb, 6], qfrc fp32 [nv]; either may be NULL),
 // read by every later emu_step / emu_forward from the caller's memory
 void emu_set_applied(EmuBase* s, float* xfrc, float* qfrc) { s->ap.xfrc = xfrc; s->ap.qfrc = qfrc; }
+// body outputs of the emulated env's current state (locosim_set_body_outputs): fp32 [nb, LS_BODY_DIM] into `out`
+void emu_body_outputs(EmuBase* s, float* out) { s->body(out); }
 long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, 0}; return v[k]; }
 long emu_ls_evals() { return g_ls_evals; }
 long emu_ls_searches() { return g_ls_searches; }

@@ -82,6 +82,8 @@ def load_library():
     lib.locosim_nbody.argtypes = [vp]
     lib.locosim_set_applied_forces.restype = ip
     lib.locosim_set_applied_forces.argtypes = [vp, vp, vp]
+    lib.locosim_set_body_outputs.restype = ip
+    lib.locosim_set_body_outputs.argtypes = [vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -93,7 +95,12 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_kernels_per_step", "locosim_reset_rows", "locosim_set_goal", "locosim_measure_fp32_peak",
                     "locosim_set_reset_rotation", "locosim_get_cursor", "locosim_dataset_rows", "locosim_create_dataset",
                     "locosim_debug_counters", "locosim_set_timeline", "locosim_set_time_limit",
-                    "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces"]
+                    "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
+                    "locosim_set_body_outputs"]
+
+# values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
+# linear velocity of the body-frame origin (3), world frame
+BODY_DIM = 13
 
 # bits of the done byte of a step (include/locosim.h)
 DONE_ABSORBING, DONE_TRUNCATED = 1, 2
@@ -164,6 +171,7 @@ class CudaEngine:
         self.nq = self.lib.locosim_nq(h)
         self.nbody = self.lib.locosim_nbody(h)
         self._applied = (None, None)      # the registered applied-force tensors (kept alive while registered)
+        self._body_out = (None, None)     # the registered body-output tensors (likewise)
         # obs / reward / done of a step live in ONE device allocation (three views), so that a consumer on the host can
         # fetch the whole step result with a single D2H copy of `packed_out`
         N, D = int(n_envs), self.obs_dim
@@ -207,7 +215,7 @@ class CudaEngine:
             self._check(self.lib.locosim_set_reset_rotation(self.h, _ptr(rot_angle)))
         self._check(self.lib.locosim_reset_rows(self.h, _ptr(mask), _ptr(traj_no), _ptr(step_no), _ptr(pool_row), _ptr(out),
                                                 self._stream()))
-        self.launches += 1
+        self.launches += 1 if self._body_out[1] is None else 2
         return out
 
     @property
@@ -271,6 +279,27 @@ class CudaEngine:
                 raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
         self._check(self.lib.locosim_set_applied_forces(self.h, _ptr(xfrc), _ptr(qfrc)))
         self._applied = (xfrc, qfrc)
+
+    def set_body_outputs(self, body=None, next_body=None):
+        """Register the body outputs of include/locosim.h (MuJoCo's xpos / xquat / body velocity): `body` and `next_body`
+        float32 cuda [n_envs, nbody, BODY_DIM], either None. Every step writes `body` for the state `obs` describes (zeros for
+        a non-finite env) and `next_body` for the state to act on next (after the auto-reset); reset() and set_state() write
+        `next_body` as well. The engine keeps a reference to them. None, None turns the feature off. Register outside of
+        CUDA-graph capture, and capture a step again after turning the feature on: whether a step writes the rows is fixed
+        when it is captured (a graph captured with nothing registered writes only the terminal rows of the envs it resets;
+        one captured with buffers registered writes into whatever buffers are registered at each replay)."""
+        t = self.torch
+        shape = (self.n_envs, self.nbody, BODY_DIM)
+        for x, name in ((body, "body"), (next_body, "next_body")):
+            if x is None:
+                continue
+            if x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
+                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+            if tuple(x.shape) != shape:
+                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+        self._check(self.lib.locosim_set_body_outputs(self.h, _ptr(body), _ptr(next_body)))
+        self._body_out = (body, next_body)
+        self.kernels_per_step = self.lib.locosim_kernels_per_step(self.h)     # (+1 while registered: body_kernel)
 
     def episode_stats(self):
         """(length int32, return float32, last_length, last_return), each [n_envs]: the running episode's control steps and

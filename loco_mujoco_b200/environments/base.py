@@ -238,6 +238,9 @@ class LocoEnv:
         # applied forces (xfrc_applied / qfrc_applied below): allocated and registered with the engine on first access
         self._xfrc_applied = None
         self._qfrc_applied = None
+        # body outputs (body_state / next_body_state below): allocated and registered with the engine on first access
+        self._body_state = None
+        self._next_body_state = None
         self._engine = None
         self._obs = None
 
@@ -430,14 +433,17 @@ class LocoEnv:
                 self._engine.set_time_limit(self._max_episode_steps, self._truncate_at_trajectory_end)
             if self._xfrc_applied is not None or self._qfrc_applied is not None:
                 self._engine.set_applied_forces(self._xfrc_applied, self._qfrc_applied)
+            if self._body_state is not None:
+                self._engine.set_body_outputs(self._body_state, self._next_body_state)
         return self._engine
 
     # ---------------------------------------------------------------------------------------------------
     # applied forces (MuJoCo's mjData.xfrc_applied / qfrc_applied, include/locosim.h locosim_set_applied_forces)
     # ---------------------------------------------------------------------------------------------------
     def body_index(self, name):
-        """Row of body `name` in `xfrc_applied` (an index of the compiled model). ValueError for an unknown name and for a
-        body that fuse_static merged into its parent; the message then names the parent."""
+        """Row of body `name` in `xfrc_applied`, `body_state` and `next_body_state` (an index of the compiled model).
+        ValueError for an unknown name and for a body that fuse_static merged into its parent; the message then names the
+        parent."""
         return self._model.body_index(name)
 
     @property
@@ -467,6 +473,41 @@ class LocoEnv:
         x, q = (t, self._qfrc_applied) if len(shape) == 3 else (self._xfrc_applied, t)
         eng.set_applied_forces(x, q)
         return t
+
+    # ---------------------------------------------------------------------------------------------------
+    # body outputs (MuJoCo's xpos / xquat / mj_objectVelocity, include/locosim.h locosim_set_body_outputs)
+    # ---------------------------------------------------------------------------------------------------
+    @property
+    def body_state(self):
+        """float32 torch tensor [num_envs, nbody, BODY_DIM = 13] on the env's device, rewritten by every step: per body (row
+        `body_index(name)`) the world position of the body frame (3), its orientation quaternion w, x, y, z (4), its angular
+        velocity (3) and the linear velocity of the body-frame origin (3), both in world coordinates (mj_objectVelocity with
+        mjOBJ_XBODY: the frame origin, not the centre of mass). It describes the state the step's observation describes: for
+        an env that ended, its terminal state; for an env whose state became non-finite, zeros. Values are those of an
+        mj_forward on that state (MuJoCo's mjData after mj_step still holds the start of the last sub-step). Allocated and
+        registered, together with `next_body_state`, on first access of either: an env that never touches them computes
+        nothing extra. Touch them before capturing a step in a CUDA graph: a graph captured before the first access does
+        not write them (capture it again afterwards)."""
+        if self._body_state is None:
+            self._new_body_outputs()
+        return self._body_state
+
+    @property
+    def next_body_state(self):
+        """Like `body_state`, for the state the env acts from next: after a step's auto-reset (rows of envs that did not
+        reset equal `body_state`), after reset() and after reset(obs=...)."""
+        if self._next_body_state is None:
+            self._new_body_outputs()
+        return self._next_body_state
+
+    def _new_body_outputs(self):
+        import torch
+        from ..engine import BODY_DIM
+        eng = self._get_engine()
+        shape = (self.num_envs, self._model.nbody, BODY_DIM)
+        self._body_state = torch.zeros(shape, dtype=torch.float32, device=eng.device)
+        self._next_body_state = torch.zeros(shape, dtype=torch.float32, device=eng.device)
+        eng.set_body_outputs(self._body_state, self._next_body_state)
 
     # ---------------------------------------------------------------------------------------------------
     # the hot path

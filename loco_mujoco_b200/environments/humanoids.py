@@ -300,6 +300,14 @@ class HumanoidTorque4AgesAll:
     qfrc_applied = property(_no_applied_forces)
     body_index = _no_applied_forces
 
+    # ---- body outputs: for the same reason ----
+    def _no_body_outputs(self, *args):
+        raise NotImplementedError("body outputs (body_state / next_body_state) are not available for HumanoidTorque4Ages "
+                                  "mode 'all': use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
+
+    body_state = property(_no_body_outputs)
+    next_body_state = property(_no_body_outputs)
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch
