@@ -170,6 +170,207 @@ __device__ __forceinline__ void append_env(const SplitState& split, int wr, int 
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// Per-env parts of a control step shared by the fused (step_kernel), sub-step (substep_kernel) and persistent
+// (persist_kernel) kernels: the block's pair-table staging, the reward of the previous observation, the carry record
+// between the launches or chunks of a split step, and the end of the step. Each kernel keeps only what differs: how a warp
+// finds its env, which sub-steps it runs, and where the env goes next. tests/test_substep_launches.py and
+// tests/test_persistent_kernel.py hold the three kernels to the same bits.
+// ----------------------------------------------------------------------------------------------------------
+
+// LOCOSIM_STAGE (default on where it fits): the table of the PRIMITIVE candidate pairs of the mid-phase (packed geom pair +
+// bound; UnitreeA1: 357 entries read in every dynamics evaluation by every warp) is staged once per block into the shared
+// memory behind the per-env working sets by ONE TMA bulk copy (cp.async.bulk global -> shared::cta, completion on an
+// mbarrier); EnvS::pk_tab points to it, DevModel::pk_n is its entry count. Called by the whole block.
+template <class C>
+__device__ __forceinline__ void stage_pair_table(unsigned char* smem_raw, const unsigned char* __restrict__ stage_src,
+                                                 int stage_bytes) {
+  if (stage_bytes <= 0) return;
+  unsigned char* dst = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
+  const unsigned dst_a = (unsigned)__cvta_generic_to_shared(dst);
+  const unsigned bar_a = dst_a + (unsigned)stage_bytes;
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"((unsigned)stage_bytes) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
+                 "l"(stage_src), "r"((unsigned)stage_bytes), "r"(bar_a)
+                 : "memory");
+  }
+  __syncthreads();                                    // (the barrier object is initialised before anybody polls it)
+  unsigned ok = 0;
+  while (!ok)
+    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                 : "=r"(ok) : "r"(bar_a) : "memory");
+}
+
+// reward depends on the *previous* observation only (utils/reward.py via base.py:170-176): evaluated before the physics
+// (the tracking reward, which compares the new observation with the mocap table, is step_epilogue's)
+template <class C>
+__device__ __forceinline__ float prev_obs_reward(const DevTask& t, const EnvS<C>& e) {
+  float rew = 0;
+  if (t.reward_type == LS_REWARD_TARGET_VELOCITY) { float d = obs_value(t, e, t.ri[0]) - t.rp[0]; rew = expf(-d * d); }
+  else if (t.reward_type == LS_REWARD_VELOCITY_VECTOR) {
+    float g = obs_value(t, e, t.ri[3]);
+    float dx = obs_value(t, e, t.ri[0]) - g * obs_value(t, e, t.ri[2]);
+    float dy = obs_value(t, e, t.ri[1]) - g * obs_value(t, e, t.ri[2] + 1);
+    rew = expf(-5.0f * sqrtf(dx * dx + dy * dy));
+  } else if (t.reward_type == LS_REWARD_POS) rew = obs_value(t, e, t.ri[0]);
+  return rew;
+}
+
+// carry record of an env (LS_CARRY words): what the fused kernel keeps in shared memory across sub-steps and
+// init_workspace clears, and the reward of the previous observation; stored by the whole warp after a launch or chunk that
+// is not the last of the control step, loaded by the next one. CG: read past L1 (the persistent kernel: another SM of the
+// same launch may have written the record).
+template <class C>
+__device__ __forceinline__ void save_carry(int* carry, const EnvS<C>& e, float rew) {
+  static_assert(EnvS<C>::NSEP <= 4 && 3 * LS_MAX_GRF <= 12, "carry record layout");
+  const int lane = threadIdx.x & 31;
+  if (lane == 0) { carry[0] = e.iter_sum; carry[1] = e.mpr_calls; carry[2] = e.sep_next; carry[3] = __float_as_int(rew); }
+  if (lane < EnvS<C>::NSEP) carry[4 + lane] = e.sep_pair[lane];
+  if (lane < 3 * EnvS<C>::NSEP) carry[8 + lane] = __float_as_int((&e.sep_dir[0][0])[lane]);
+  if (lane < 3 * LS_MAX_GRF) carry[20 + lane] = __float_as_int(e.grf[lane]);
+}
+template <bool CG>
+__device__ __forceinline__ int ld_carry(const int* p) {
+  if constexpr (CG) return __ldcg(p);
+  else return *p;
+}
+// returns the carried reward (lane 0; 0 on the other lanes)
+template <class C, bool CG>
+__device__ __forceinline__ float load_carry(const int* carry, EnvS<C>& e) {
+  const int lane = threadIdx.x & 31;
+  float rew = 0;
+  if (lane == 0) {
+    e.iter_sum = ld_carry<CG>(&carry[0]); e.mpr_calls = ld_carry<CG>(&carry[1]); e.sep_next = ld_carry<CG>(&carry[2]);
+    rew = __int_as_float(ld_carry<CG>(&carry[3]));
+  }
+  if (lane < EnvS<C>::NSEP) e.sep_pair[lane] = ld_carry<CG>(&carry[4 + lane]);
+  if (lane < 3 * EnvS<C>::NSEP) (&e.sep_dir[0][0])[lane] = __int_as_float(ld_carry<CG>(&carry[8 + lane]));
+  if (lane < 3 * LS_MAX_GRF) e.grf[lane] = __int_as_float(ld_carry<CG>(&carry[20 + lane]));
+  __syncwarp();
+  return rew;
+}
+
+// end of the control step of one (not ghost) env, by its warp: observation, termination, tracking reward and cursor, time
+// limit, episode statistics, counters and regrouping key, auto-reset, state store. Returns whether the env was reset.
+template <class C>
+__device__ __forceinline__ bool step_epilogue(int ms, const DevTask& t, const EngineState& st, EnvS<C>& e, int env, float rew,
+                                              float* __restrict__ obs, float* __restrict__ reward,
+                                              uint8_t* __restrict__ done, float* __restrict__ next_obs, int auto_reset,
+                                              uint64_t seed, int64_t env_off, int key_mode_in) {
+  const int lane = threadIdx.x & 31;
+  int key_mode = key_mode_in & 0xffff;
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv, D = t.obs_dim;
+
+  // ---- observation, termination, reward ----
+  bool bad = false;
+  for (int i = lane; i < nv; i += 32) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+  bool fallen = false;
+  for (int k = lane; k < t.n_done; k += 32) {
+    float v = obs_value(t, e, t.done_obs_idx[k]);
+    fallen |= (v < t.done_lo[k]) || (v > t.done_hi[k]);
+  }
+  bad = __any_sync(0xffffffffu, bad);
+  fallen = __any_sync(0xffffffffu, fallen) && t.use_absorbing;
+  const bool is_done = fallen || bad;
+  if (t.reward_type == LS_REWARD_TRACKING) {
+    // mocap-tracking reward (include/locosim_task.h): the cursor advances one sample, the observation reached by this step
+    // is compared with the table row at the advanced cursor
+    int cur = st.cursor[env];
+    const int tj = cur / t.traj_len;
+    int sp = cur - tj * t.traj_len;
+    sp = sp + 1 < t.traj_len ? sp + 1 : t.traj_len - 1;
+    cur = tj * t.traj_len + sp;
+    const float* ref = t.table + (size_t)cur * (2 * nv + t.n_goal);
+    float ep = 0, ev = 0;
+    for (int k = lane; k < D; k += 32) {
+      const int ty = t.obs_src_type[k], idx = t.obs_src_idx[k];
+      if (ty == LS_OBS_QPOS) { const float d = e.qpos[idx] - ref[idx]; ep += d * d; }
+      else if (ty == LS_OBS_QVEL) { const float d = e.qvel[idx] - ref[nv + idx]; ev += d * d; }
+    }
+    ep = warp_sum(ep); ev = warp_sum(ev);
+    rew = bad ? 0.0f : t.track[0] * expf(-t.track[1] * ep) + t.track[2] * expf(-t.track[3] * ev);
+    if (lane == 0) st.cursor[env] = cur;
+  }
+  for (int k = lane; k < D; k += 32) {
+    float v = obs_value(t, e, k);
+    if (bad) v = 0.0f;
+    obs[(size_t)env * D + k] = v;
+  }
+  bool truncated = false;
+  if (lane == 0) {
+    float r = rew;
+    reward[env] = r;
+    // episode statistics and time limit (include/locosim.h): length and return of the running episode, the two limits,
+    // bit 1 of the done byte (absorbing wins), the finished episode's numbers
+    int4 es = st.ep[env];
+    es.x += 1; es.y = __float_as_int(__int_as_float(es.y) + r);
+    truncated = st.max_episode_steps > 0 && es.x >= st.max_episode_steps;
+    if (st.end_of_trajectory) {
+      // one (clamped) advance of the cursor per step: the tracking reward above has made it already
+      const int cur = st.cursor[env];
+      int sp = cur % t.traj_len;
+      if (t.reward_type != LS_REWARD_TRACKING && sp + 1 < t.traj_len) { sp += 1; st.cursor[env] = cur + 1; }
+      truncated |= sp == t.traj_len - 1;
+    }
+    truncated = truncated && !is_done;
+    done[env] = is_done ? 1 : (truncated ? 2 : 0);
+    if (is_done || truncated) { es.z = es.x; es.w = es.y; }
+    st.ep[env] = es;
+    int* cnt = st.counters + (size_t)env * 8;
+    cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
+    if (bad) cnt[4] += 1;
+    {
+      int key = e.iter_sum;
+      const int mpr_w = (key_mode >> 8) & 255;           // weight of one MPR run in Newton-iteration units
+      key_mode &= 255;
+      if (key_mode == 1) key = (cnt[5] + e.iter_sum + 1) >> 1;
+      else if (key_mode == 2) key = e.solver_iter * 8;
+      else if (key_mode == 3) key = e.iter_sum + (e.nefc >> 1) + mpr_w * min(e.mpr_calls, 64);
+      else if (key_mode == 4) key = (3 * cnt[5] + e.iter_sum + 2) >> 2;
+      else if (key_mode == 5) key = e.iter_sum + 4 * e.solver_iter;
+      else if (key_mode == 6) key = e.iter_sum + e.nefc;
+      else if (key_mode == 7) key = e.iter_sum + 4 * e.solver_iter + (e.nefc >> 1);
+      cnt[5] = key;
+    } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
+  }
+
+  // ---- auto-reset (reset_env is a whole-warp call: lane 0's verdict on the time limit goes to every lane first) ----
+  truncated = __shfl_sync(0xffffffffu, (int)truncated, 0) != 0;
+  const bool reset = (is_done || truncated) && (auto_reset || bad);
+  if (reset) {
+    const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
+    int ep = st.episode[env];
+    int tr, sp;
+    draw_reset(seed, env_off + env, ep, t.n_traj, t.traj_len, &tr, &sp);
+    __syncwarp();
+    reset_env(ms, t, e, tr, sp, t.rot[0] >= 0 ? draw_rot_angle(seed, env_off + env, ep) : 0.0f);
+    if (lane == 0) {
+      const int prow = draw_pool_row(seed, env_off + env, ep, st.pool_K);
+      st.episode[env] = ep + 1; st.counters[(size_t)env * 8 + 1] += 1;
+      if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
+      st.dr_row[env] = prow;
+      st.cursor[env] = tr * t.traj_len + sp;
+      *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
+      e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
+    }
+    __syncwarp();
+    for (int k = lane; k < t.n_goal; k += 32) st.goal[(size_t)env * 4 + k] = e.goal[k];
+  }
+  if (next_obs) for (int k = lane; k < D; k += 32) next_obs[(size_t)env * D + k] = obs_value(t, e, k);
+
+  // ---- store state ----
+  for (int i = lane; i < nv; i += 32) {
+    st.qpos[(size_t)env * nv + i] = e.qpos[i];
+    st.qvel[(size_t)env * nv + i] = e.qvel[i];
+    st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
+  }
+  return reset;
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // step kernel: one warp per env, EnvS in dynamic shared memory
 // ----------------------------------------------------------------------------------------------------------
 template <class C>
@@ -181,29 +382,7 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
                                                     const unsigned char* __restrict__ stage_src, int stage_bytes) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int key_mode = key_mode_in & 0xffff;
-  if (stage_bytes > 0) {
-    // LOCOSIM_STAGE (default on where it fits): the table of the PRIMITIVE candidate pairs of the mid-phase (packed geom pair +
-    // bound; UnitreeA1: 357 entries read in every dynamics evaluation by every warp) is staged once per block into the shared
-    // memory behind the per-env working sets by ONE TMA bulk copy (cp.async.bulk global -> shared::cta, completion on an
-    // mbarrier); EnvS::pk_tab points to it, DevModel::pk_n is its entry count.
-    unsigned char* dst = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
-    const unsigned dst_a = (unsigned)__cvta_generic_to_shared(dst);
-    const unsigned bar_a = dst_a + (unsigned)stage_bytes;
-    if (threadIdx.x == 0) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"((unsigned)stage_bytes) : "memory");
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
-                   "l"(stage_src), "r"((unsigned)stage_bytes), "r"(bar_a)
-                   : "memory");
-    }
-    __syncthreads();                                    // (the barrier object is initialised before anybody polls it)
-    unsigned ok = 0;
-    while (!ok)
-      asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                   : "=r"(ok) : "r"(bar_a) : "memory");
-  }
+  stage_pair_table<C>(smem_raw, stage_src, stage_bytes);
   // warps past the last env shadow it (same barriers, no stores): the block-wide barriers inside the solver have
   // data-dependent counts, so every warp of a block has to run the physics
   const int slot_raw = blockIdx.x * (blockDim.x >> 5) + warp;
@@ -211,7 +390,7 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
   const int env = st.perm[ghost ? n_envs - 1 : slot_raw];
   EnvS<C>& e = reinterpret_cast<EnvS<C>*>(smem_raw)[warp];
   const DevModel& m = c_models[ms];
-  const int nv = m.nv, nu = m.nu, D = t.obs_dim;
+  const int nv = m.nv, nu = m.nu;
   if (lane == 0) {
     e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
     e.env = env;
@@ -234,15 +413,7 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
   init_workspace(ms, e);
   if (lane == 0) e.iter_sum = 0;
   if (lane < 3 * LS_MAX_GRF) e.grf[lane] = 0;
-  // reward depends on the *previous* observation only (utils/reward.py via base.py:170-176): evaluate it now
-  float rew = 0;
-  if (t.reward_type == LS_REWARD_TARGET_VELOCITY) { float d = obs_value(t, e, t.ri[0]) - t.rp[0]; rew = expf(-d * d); }
-  else if (t.reward_type == LS_REWARD_VELOCITY_VECTOR) {
-    float g = obs_value(t, e, t.ri[3]);
-    float dx = obs_value(t, e, t.ri[0]) - g * obs_value(t, e, t.ri[2]);
-    float dy = obs_value(t, e, t.ri[1]) - g * obs_value(t, e, t.ri[2] + 1);
-    rew = expf(-5.0f * sqrtf(dx * dx + dy * dy));
-  } else if (t.reward_type == LS_REWARD_POS) rew = obs_value(t, e, t.ri[0]);
+  float rew = prev_obs_reward(t, e);
 
   // ---- physics ----
   if (sync_substeps) {
@@ -253,151 +424,23 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
   }
 
   if (ghost) return;
-
-  // ---- observation, termination, reward ----
-  bool bad = false;
-  for (int i = lane; i < nv; i += 32) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
-  bool fallen = false;
-  for (int k = lane; k < t.n_done; k += 32) {
-    float v = obs_value(t, e, t.done_obs_idx[k]);
-    fallen |= (v < t.done_lo[k]) || (v > t.done_hi[k]);
-  }
-  bad = __any_sync(0xffffffffu, bad);
-  fallen = __any_sync(0xffffffffu, fallen) && t.use_absorbing;
-  const bool is_done = fallen || bad;
-  if (t.reward_type == LS_REWARD_TRACKING) {
-    // mocap-tracking reward (include/locosim_task.h): the cursor advances one sample, the observation reached by this step
-    // is compared with the table row at the advanced cursor
-    int cur = st.cursor[env];
-    const int tj = cur / t.traj_len;
-    int sp = cur - tj * t.traj_len;
-    sp = sp + 1 < t.traj_len ? sp + 1 : t.traj_len - 1;
-    cur = tj * t.traj_len + sp;
-    const float* ref = t.table + (size_t)cur * (2 * nv + t.n_goal);
-    float ep = 0, ev = 0;
-    for (int k = lane; k < D; k += 32) {
-      const int ty = t.obs_src_type[k], idx = t.obs_src_idx[k];
-      if (ty == LS_OBS_QPOS) { const float d = e.qpos[idx] - ref[idx]; ep += d * d; }
-      else if (ty == LS_OBS_QVEL) { const float d = e.qvel[idx] - ref[nv + idx]; ev += d * d; }
-    }
-    ep = warp_sum(ep); ev = warp_sum(ev);
-    rew = bad ? 0.0f : t.track[0] * expf(-t.track[1] * ep) + t.track[2] * expf(-t.track[3] * ev);
-    if (lane == 0) st.cursor[env] = cur;
-  }
-  for (int k = lane; k < D; k += 32) {
-    float v = obs_value(t, e, k);
-    if (bad) v = 0.0f;
-    obs[(size_t)env * D + k] = v;
-  }
-  bool truncated = false;
-  if (lane == 0) {
-    float r = rew;
-    reward[env] = r;
-    // episode statistics and time limit (include/locosim.h): length and return of the running episode, the two limits,
-    // bit 1 of the done byte (absorbing wins), the finished episode's numbers
-    int4 es = st.ep[env];
-    es.x += 1; es.y = __float_as_int(__int_as_float(es.y) + r);
-    truncated = st.max_episode_steps > 0 && es.x >= st.max_episode_steps;
-    if (st.end_of_trajectory) {
-      // one (clamped) advance of the cursor per step: the tracking reward above has made it already
-      const int cur = st.cursor[env];
-      int sp = cur % t.traj_len;
-      if (t.reward_type != LS_REWARD_TRACKING && sp + 1 < t.traj_len) { sp += 1; st.cursor[env] = cur + 1; }
-      truncated |= sp == t.traj_len - 1;
-    }
-    truncated = truncated && !is_done;
-    done[env] = is_done ? 1 : (truncated ? 2 : 0);
-    if (is_done || truncated) { es.z = es.x; es.w = es.y; }
-    st.ep[env] = es;
-    int* cnt = st.counters + (size_t)env * 8;
-    cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
-    if (bad) cnt[4] += 1;
-    {
-      int key = e.iter_sum;
-      const int mpr_w = (key_mode >> 8) & 255;           // weight of one MPR run in Newton-iteration units
-      key_mode &= 255;
-      if (key_mode == 1) key = (cnt[5] + e.iter_sum + 1) >> 1;
-      else if (key_mode == 2) key = e.solver_iter * 8;
-      else if (key_mode == 3) key = e.iter_sum + (e.nefc >> 1) + mpr_w * min(e.mpr_calls, 64);
-      else if (key_mode == 4) key = (3 * cnt[5] + e.iter_sum + 2) >> 2;
-      else if (key_mode == 5) key = e.iter_sum + 4 * e.solver_iter;
-      else if (key_mode == 6) key = e.iter_sum + e.nefc;
-      else if (key_mode == 7) key = e.iter_sum + 4 * e.solver_iter + (e.nefc >> 1);
-      cnt[5] = key;
-    } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
-  }
-
-  // ---- auto-reset (reset_env is a whole-warp call: lane 0's verdict on the time limit goes to every lane first) ----
-  truncated = __shfl_sync(0xffffffffu, (int)truncated, 0) != 0;
-  if ((is_done || truncated) && (auto_reset || bad)) {
-    const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
-    int ep = st.episode[env];
-    int tr, sp;
-    draw_reset(seed, env_off + env, ep, t.n_traj, t.traj_len, &tr, &sp);
-    __syncwarp();
-    reset_env(ms, t, e, tr, sp, t.rot[0] >= 0 ? draw_rot_angle(seed, env_off + env, ep) : 0.0f);
-    if (lane == 0) {
-      const int prow = draw_pool_row(seed, env_off + env, ep, st.pool_K);
-      st.episode[env] = ep + 1; st.counters[(size_t)env * 8 + 1] += 1;
-      if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
-      st.dr_row[env] = prow;
-      st.cursor[env] = tr * t.traj_len + sp;
-      *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
-      e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
-    }
-    __syncwarp();
-    for (int k = lane; k < t.n_goal; k += 32) st.goal[(size_t)env * 4 + k] = e.goal[k];
-  }
-  if (next_obs) for (int k = lane; k < D; k += 32) next_obs[(size_t)env * D + k] = obs_value(t, e, k);
-
-  // ---- store state ----
-  for (int i = lane; i < nv; i += 32) {
-    st.qpos[(size_t)env * nv + i] = e.qpos[i];
-    st.qvel[(size_t)env * nv + i] = e.qvel[i];
-    st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
-  }
+  step_epilogue<C>(ms, t, st, e, env, rew, obs, reward, done, next_obs, auto_reset, seed, env_off, key_mode_in);
 }
 
 // ----------------------------------------------------------------------------------------------------------
-// sub-step kernel body: the fused step kernel above restricted to sub-steps [k0, k1) of the control step.
-// It repeats step_kernel's staging, load, reward and epilogue on purpose: folding both into one template (or into shared
-// inline helpers) changes the code nvcc 12.9 generates for the fused kernel (sm_90a: 272 -> 260 bytes of spill stores for
-// CfgEllEuler), which is the path of every configuration that does not split. A change to one epilogue must be made to both;
-// tests/test_substep_launches.py holds them to the same bits (A1, HumanoidTorque, Talos with DR, foot forces,
-// the tracking reward, ghost warps).
+// sub-step kernel body: the fused step kernel above restricted to sub-steps [k0, k1) of the control step. Staging,
+// reward, carry record and epilogue are the shared helpers above.
 // ----------------------------------------------------------------------------------------------------------
 template <class C>
-__device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, DevTask t, SolverOpts so, EngineState st,
-                                             const float* __restrict__ action, float* __restrict__ obs,
+__device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, const DevTask& t, const SolverOpts& so,
+                                             const EngineState& st, const float* __restrict__ action, float* __restrict__ obs,
                                              float* __restrict__ reward, uint8_t* __restrict__ done,
                                              float* __restrict__ next_obs, int n_envs, int auto_reset, uint64_t seed,
                                              int64_t env_off, int sync_substeps, int key_mode_in,
                                              const unsigned char* __restrict__ stage_src, int stage_bytes, int k0, int k1,
-                                             SplitState split) {
+                                             const SplitState& split) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int key_mode = key_mode_in & 0xffff;
-  if (stage_bytes > 0) {
-    // LOCOSIM_STAGE (default on where it fits): the table of the PRIMITIVE candidate pairs of the mid-phase (packed geom pair +
-    // bound; UnitreeA1: 357 entries read in every dynamics evaluation by every warp) is staged once per block into the shared
-    // memory behind the per-env working sets by ONE TMA bulk copy (cp.async.bulk global -> shared::cta, completion on an
-    // mbarrier); EnvS::pk_tab points to it, DevModel::pk_n is its entry count.
-    unsigned char* dst = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
-    const unsigned dst_a = (unsigned)__cvta_generic_to_shared(dst);
-    const unsigned bar_a = dst_a + (unsigned)stage_bytes;
-    if (threadIdx.x == 0) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"((unsigned)stage_bytes) : "memory");
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
-                   "l"(stage_src), "r"((unsigned)stage_bytes), "r"(bar_a)
-                   : "memory");
-    }
-    __syncthreads();                                    // (the barrier object is initialised before anybody polls it)
-    unsigned ok = 0;
-    while (!ok)
-      asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                   : "=r"(ok) : "r"(bar_a) : "memory");
-  }
+  stage_pair_table<C>(smem_raw, stage_src, stage_bytes);
   // warps past the last env shadow it (same barriers, no stores): the block-wide barriers inside the solver have
   // data-dependent counts, so every warp of a block has to run the physics
   const int slot_raw = blockIdx.x * (blockDim.x >> 5) + warp;
@@ -409,7 +452,7 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
                                 : slot;
   EnvS<C>& e = reinterpret_cast<EnvS<C>*>(smem_raw)[warp];
   const DevModel& m = c_models[ms];
-  const int nv = m.nv, nu = m.nu, D = t.obs_dim;
+  const int nv = m.nv, nu = m.nu;
   if (lane == 0) {
     e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
     e.env = env;
@@ -430,29 +473,15 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
   if (lane < 4) e.goal[lane] = st.goal[(size_t)env * 4 + lane];
   __syncwarp();
   init_workspace(ms, e);
-  float rew = 0;
   int* carry = split.carry + (size_t)env * LS_CARRY;
-  static_assert(EnvS<C>::NSEP <= 4 && 3 * LS_MAX_GRF <= 12, "carry record layout");
+  float rew;
   if (k0 > 0) {
-    // what the previous launches of this control step left behind (init_workspace above cleared part of it)
-    if (lane == 0) { e.iter_sum = carry[0]; e.mpr_calls = carry[1]; e.sep_next = carry[2]; rew = __int_as_float(carry[3]); }
-    if (lane < EnvS<C>::NSEP) e.sep_pair[lane] = carry[4 + lane];
-    if (lane < 3 * EnvS<C>::NSEP) (&e.sep_dir[0][0])[lane] = __int_as_float(carry[8 + lane]);
-    if (lane < 3 * LS_MAX_GRF) e.grf[lane] = __int_as_float(carry[20 + lane]);
-    __syncwarp();
+    rew = load_carry<C, false>(carry, e);   // what the previous launches of this control step left behind
   } else {
     if (lane == 0) e.iter_sum = 0;
     if (lane < 3 * LS_MAX_GRF) e.grf[lane] = 0;
-    // reward depends on the *previous* observation only (utils/reward.py via base.py:170-176): evaluate it now
-    if (t.reward_type == LS_REWARD_TARGET_VELOCITY) { float d = obs_value(t, e, t.ri[0]) - t.rp[0]; rew = expf(-d * d); }
-    else if (t.reward_type == LS_REWARD_VELOCITY_VECTOR) {
-      float g = obs_value(t, e, t.ri[3]);
-      float dx = obs_value(t, e, t.ri[0]) - g * obs_value(t, e, t.ri[2]);
-      float dy = obs_value(t, e, t.ri[1]) - g * obs_value(t, e, t.ri[2] + 1);
-      rew = expf(-5.0f * sqrtf(dx * dx + dy * dy));
-    } else if (t.reward_type == LS_REWARD_POS) rew = obs_value(t, e, t.ri[0]);
+    rew = prev_obs_reward(t, e);
   }
-  const int iter0 = e.iter_sum, mpr0 = e.mpr_calls;    // (the regrouping key counts this launch's sub-steps)
 
   // ---- physics ----
   if (sync_substeps) {
@@ -461,6 +490,10 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
   } else {
     physics_substeps(ms, e, so, k1 - k0, t.grf_group, t.n_grf);
   }
+  // the regrouping key counts this launch's sub-steps: the counts at its start are those of the carry record, which the
+  // warp rewrites only below (0 in the first launch; reading them here rather than keeping them live across the physics
+  // keeps this kernel's stack within the fused kernel's)
+  int key = launch_key(t, e, k0, k1, k0 > 0 ? carry[0] : 0, k0 > 0 ? carry[1] : 0, key_mode_in);
 
   if (k1 < t.n_substeps) {
     // ---- not the last launch of the control step: state and carried fields to HBM, env into its bucket ----
@@ -470,121 +503,16 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, De
         st.qvel[(size_t)env * nv + i] = e.qvel[i];
         st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
       }
-      if (lane == 0) { carry[0] = e.iter_sum; carry[1] = e.mpr_calls; carry[2] = e.sep_next; carry[3] = __float_as_int(rew); }
-      if (lane < EnvS<C>::NSEP) carry[4 + lane] = e.sep_pair[lane];
-      if (lane < 3 * EnvS<C>::NSEP) carry[8 + lane] = __float_as_int((&e.sep_dir[0][0])[lane]);
-      if (lane < 3 * LS_MAX_GRF) carry[20 + lane] = __float_as_int(e.grf[lane]);
-      if (lane == 0 && split.regroup) append_env(split, rd ^ 1, env, n_envs, launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in));
+      save_carry<C>(carry, e, rew);
+      if (lane == 0 && split.regroup) append_env(split, rd ^ 1, env, n_envs, key);
     }
     return;
   }
   if (ghost) return;
-
-  // ---- observation, termination, reward ----
-  bool bad = false;
-  for (int i = lane; i < nv; i += 32) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
-  bool fallen = false;
-  for (int k = lane; k < t.n_done; k += 32) {
-    float v = obs_value(t, e, t.done_obs_idx[k]);
-    fallen |= (v < t.done_lo[k]) || (v > t.done_hi[k]);
-  }
-  bad = __any_sync(0xffffffffu, bad);
-  fallen = __any_sync(0xffffffffu, fallen) && t.use_absorbing;
-  const bool is_done = fallen || bad;
-  if (t.reward_type == LS_REWARD_TRACKING) {
-    // mocap-tracking reward (include/locosim_task.h): the cursor advances one sample, the observation reached by this step
-    // is compared with the table row at the advanced cursor
-    int cur = st.cursor[env];
-    const int tj = cur / t.traj_len;
-    int sp = cur - tj * t.traj_len;
-    sp = sp + 1 < t.traj_len ? sp + 1 : t.traj_len - 1;
-    cur = tj * t.traj_len + sp;
-    const float* ref = t.table + (size_t)cur * (2 * nv + t.n_goal);
-    float ep = 0, ev = 0;
-    for (int k = lane; k < D; k += 32) {
-      const int ty = t.obs_src_type[k], idx = t.obs_src_idx[k];
-      if (ty == LS_OBS_QPOS) { const float d = e.qpos[idx] - ref[idx]; ep += d * d; }
-      else if (ty == LS_OBS_QVEL) { const float d = e.qvel[idx] - ref[nv + idx]; ev += d * d; }
-    }
-    ep = warp_sum(ep); ev = warp_sum(ev);
-    rew = bad ? 0.0f : t.track[0] * expf(-t.track[1] * ep) + t.track[2] * expf(-t.track[3] * ev);
-    if (lane == 0) st.cursor[env] = cur;
-  }
-  for (int k = lane; k < D; k += 32) {
-    float v = obs_value(t, e, k);
-    if (bad) v = 0.0f;
-    obs[(size_t)env * D + k] = v;
-  }
-  bool truncated = false;
-  if (lane == 0) {
-    float r = rew;
-    reward[env] = r;
-    // episode statistics and time limit (include/locosim.h): length and return of the running episode, the two limits,
-    // bit 1 of the done byte (absorbing wins), the finished episode's numbers
-    int4 es = st.ep[env];
-    es.x += 1; es.y = __float_as_int(__int_as_float(es.y) + r);
-    truncated = st.max_episode_steps > 0 && es.x >= st.max_episode_steps;
-    if (st.end_of_trajectory) {
-      // one (clamped) advance of the cursor per step: the tracking reward above has made it already
-      const int cur = st.cursor[env];
-      int sp = cur % t.traj_len;
-      if (t.reward_type != LS_REWARD_TRACKING && sp + 1 < t.traj_len) { sp += 1; st.cursor[env] = cur + 1; }
-      truncated |= sp == t.traj_len - 1;
-    }
-    truncated = truncated && !is_done;
-    done[env] = is_done ? 1 : (truncated ? 2 : 0);
-    if (is_done || truncated) { es.z = es.x; es.w = es.y; }
-    st.ep[env] = es;
-    int* cnt = st.counters + (size_t)env * 8;
-    cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
-    if (bad) cnt[4] += 1;
-    {
-      int key = e.iter_sum;
-      const int mpr_w = (key_mode >> 8) & 255;           // weight of one MPR run in Newton-iteration units
-      key_mode &= 255;
-      if (key_mode == 1) key = (cnt[5] + e.iter_sum + 1) >> 1;
-      else if (key_mode == 2) key = e.solver_iter * 8;
-      else if (key_mode == 3) key = e.iter_sum + (e.nefc >> 1) + mpr_w * min(e.mpr_calls, 64);
-      else if (key_mode == 4) key = (3 * cnt[5] + e.iter_sum + 2) >> 2;
-      else if (key_mode == 5) key = e.iter_sum + 4 * e.solver_iter;
-      else if (key_mode == 6) key = e.iter_sum + e.nefc;
-      else if (key_mode == 7) key = e.iter_sum + 4 * e.solver_iter + (e.nefc >> 1);
-      cnt[5] = key;
-    } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
-  }
-
-  // ---- auto-reset (reset_env is a whole-warp call: lane 0's verdict on the time limit goes to every lane first) ----
-  truncated = __shfl_sync(0xffffffffu, (int)truncated, 0) != 0;
-  if ((is_done || truncated) && (auto_reset || bad)) {
-    const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
-    int ep = st.episode[env];
-    int tr, sp;
-    draw_reset(seed, env_off + env, ep, t.n_traj, t.traj_len, &tr, &sp);
-    __syncwarp();
-    reset_env(ms, t, e, tr, sp, t.rot[0] >= 0 ? draw_rot_angle(seed, env_off + env, ep) : 0.0f);
-    if (lane == 0) {
-      const int prow = draw_pool_row(seed, env_off + env, ep, st.pool_K);
-      st.episode[env] = ep + 1; st.counters[(size_t)env * 8 + 1] += 1;
-      if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
-      st.dr_row[env] = prow;
-      st.cursor[env] = tr * t.traj_len + sp;
-      *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
-      e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
-    }
-    __syncwarp();
-    for (int k = lane; k < t.n_goal; k += 32) st.goal[(size_t)env * 4 + k] = e.goal[k];
-  }
-  if (next_obs) for (int k = lane; k < D; k += 32) next_obs[(size_t)env * D + k] = obs_value(t, e, k);
-
-  // ---- store state ----
-  for (int i = lane; i < nv; i += 32) {
-    st.qpos[(size_t)env * nv + i] = e.qpos[i];
-    st.qvel[(size_t)env * nv + i] = e.qvel[i];
-    st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
-  }
+  const bool reset = step_epilogue<C>(ms, t, st, e, env, rew, obs, reward, done, next_obs, auto_reset, seed, env_off,
+                                      key_mode_in);
   if (lane == 0 && split.regroup) {
-    int key = launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in);
-    if ((is_done || truncated) && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
+    if (reset && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
     append_env(split, rd ^ 1, env, n_envs, key);
   }
 }
@@ -630,7 +558,7 @@ __global__ void __launch_bounds__(512, 1) substep_kernel(int ms, DevTask t, Solv
 // No grid barrier and no co-residency assumption: a block only waits for envs that running blocks hold, so the kernel
 // makes progress with any number of resident blocks.
 //
-// The body repeats substep_body on purpose (see the note there: folding changes the other kernels' code).
+// The per-env body shares the staging, reward, carry record and epilogue of the other step kernels (helpers above).
 // ----------------------------------------------------------------------------------------------------------
 #define LS_TL_WORDS 8     // timeline record: smid, chunk, envs, pop start, group start, group end (ns), iterations sum, max
 struct PersistQueue {
@@ -758,11 +686,10 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
                                             const PersistQueue& q, int par) {
   PH_T0(t_ph);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int key_mode = key_mode_in & 0xffff;
   const int k0 = c * q.chunk, k1 = min(k0 + q.chunk, t.n_substeps);
   EnvS<C>& e = reinterpret_cast<EnvS<C>*>(smem_raw)[warp];
   const DevModel& m = c_models[ms];
-  const int nv = m.nv, nu = m.nu, D = t.obs_dim;
+  const int nv = m.nv, nu = m.nu;
   e.env = env;     // (every lane: a predicated store costs the persistent kernel a spill)
   if (lane == 0) {
     e.prm = st.pool + (size_t)__ldcg(&st.dr_row[env]) * m.pool_P;
@@ -783,32 +710,15 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
   if (lane < 4) e.goal[lane] = __ldcg(&st.goal[(size_t)env * 4 + lane]);
   __syncwarp();
   init_workspace(ms, e);
-  float rew = 0;
-  int* carry = q.carry + (size_t)env * LS_CARRY;
-  static_assert(EnvS<C>::NSEP <= 4 && 3 * LS_MAX_GRF <= 12, "carry record layout");
+  float rew;
   if (k0 > 0) {
-    // what the previous chunks of this control step left behind (init_workspace above cleared part of it)
-    if (lane == 0) {
-      e.iter_sum = __ldcg(&carry[0]); e.mpr_calls = __ldcg(&carry[1]); e.sep_next = __ldcg(&carry[2]);
-      rew = __int_as_float(__ldcg(&carry[3]));
-    }
-    if (lane < EnvS<C>::NSEP) e.sep_pair[lane] = __ldcg(&carry[4 + lane]);
-    if (lane < 3 * EnvS<C>::NSEP) (&e.sep_dir[0][0])[lane] = __int_as_float(__ldcg(&carry[8 + lane]));
-    if (lane < 3 * LS_MAX_GRF) e.grf[lane] = __int_as_float(__ldcg(&carry[20 + lane]));
-    __syncwarp();
+    // what the previous chunks of this control step left behind
+    rew = load_carry<C, true>(q.carry + (size_t)env * LS_CARRY, e);
   } else {
     if (lane == 0) e.iter_sum = 0;
     if (lane < 3 * LS_MAX_GRF) e.grf[lane] = 0;
-    // reward depends on the *previous* observation only (utils/reward.py via base.py:170-176): evaluate it now
-    if (t.reward_type == LS_REWARD_TARGET_VELOCITY) { float d = obs_value(t, e, t.ri[0]) - t.rp[0]; rew = expf(-d * d); }
-    else if (t.reward_type == LS_REWARD_VELOCITY_VECTOR) {
-      float g = obs_value(t, e, t.ri[3]);
-      float dx = obs_value(t, e, t.ri[0]) - g * obs_value(t, e, t.ri[2]);
-      float dy = obs_value(t, e, t.ri[1]) - g * obs_value(t, e, t.ri[2] + 1);
-      rew = expf(-5.0f * sqrtf(dx * dx + dy * dy));
-    } else if (t.reward_type == LS_REWARD_POS) rew = obs_value(t, e, t.ri[0]);
+    rew = prev_obs_reward(t, e);
   }
-  const int iter0 = e.iter_sum, mpr0 = e.mpr_calls;    // (the regrouping key counts this chunk's sub-steps)
   PH_LAP(PH_PROLOGUE, t_ph);
   PH_CNT(PH_GROUPS, 1);
 
@@ -819,7 +729,12 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
   } else {
     physics_substeps(ms, e, so, k1 - k0, t.grf_group, t.n_grf);
   }
+  // the counts at the chunk's start, read from the carry record as in substep_body (past L1, like every read of a record
+  // another SM may have written)
+  const int* rec = q.carry + (size_t)env * LS_CARRY;
+  const int iter0 = k0 > 0 ? ld_relaxed(&rec[0]) : 0, mpr0 = k0 > 0 ? ld_relaxed(&rec[1]) : 0;
   const int iters = e.iter_sum - iter0;
+  int key = launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in);
   PH_T0(t_epi);
 
   if (k1 < t.n_substeps) {
@@ -830,127 +745,22 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
         st.qvel[(size_t)env * nv + i] = e.qvel[i];
         st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
       }
-      if (lane == 0) { carry[0] = e.iter_sum; carry[1] = e.mpr_calls; carry[2] = e.sep_next; carry[3] = __float_as_int(rew); }
-      if (lane < EnvS<C>::NSEP) carry[4 + lane] = e.sep_pair[lane];
-      if (lane < 3 * EnvS<C>::NSEP) carry[8 + lane] = __float_as_int((&e.sep_dir[0][0])[lane]);
-      if (lane < 3 * LS_MAX_GRF) carry[20 + lane] = __float_as_int(e.grf[lane]);
+      save_carry<C>(q.carry + (size_t)env * LS_CARRY, e, rew);
       __threadfence();
       __syncwarp();
-      if (lane == 0) persist_publish(q, par, c + 1, env, n_envs, launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in));
+      if (lane == 0) persist_publish(q, par, c + 1, env, n_envs, key);
     }
     PH_LAP(PH_EPILOGUE, t_epi);
     return iters;
   }
   if (ghost) return iters;
-
-  // ---- observation, termination, reward ----
-  bool bad = false;
-  for (int i = lane; i < nv; i += 32) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
-  bool fallen = false;
-  for (int k = lane; k < t.n_done; k += 32) {
-    float v = obs_value(t, e, t.done_obs_idx[k]);
-    fallen |= (v < t.done_lo[k]) || (v > t.done_hi[k]);
-  }
-  bad = __any_sync(0xffffffffu, bad);
-  fallen = __any_sync(0xffffffffu, fallen) && t.use_absorbing;
-  const bool is_done = fallen || bad;
-  if (t.reward_type == LS_REWARD_TRACKING) {
-    // mocap-tracking reward (include/locosim_task.h): the cursor advances one sample, the observation reached by this step
-    // is compared with the table row at the advanced cursor
-    int cur = st.cursor[env];
-    const int tj = cur / t.traj_len;
-    int sp = cur - tj * t.traj_len;
-    sp = sp + 1 < t.traj_len ? sp + 1 : t.traj_len - 1;
-    cur = tj * t.traj_len + sp;
-    const float* ref = t.table + (size_t)cur * (2 * nv + t.n_goal);
-    float ep = 0, ev = 0;
-    for (int k = lane; k < D; k += 32) {
-      const int ty = t.obs_src_type[k], idx = t.obs_src_idx[k];
-      if (ty == LS_OBS_QPOS) { const float d = e.qpos[idx] - ref[idx]; ep += d * d; }
-      else if (ty == LS_OBS_QVEL) { const float d = e.qvel[idx] - ref[nv + idx]; ev += d * d; }
-    }
-    ep = warp_sum(ep); ev = warp_sum(ev);
-    rew = bad ? 0.0f : t.track[0] * expf(-t.track[1] * ep) + t.track[2] * expf(-t.track[3] * ev);
-    if (lane == 0) st.cursor[env] = cur;
-  }
-  for (int k = lane; k < D; k += 32) {
-    float v = obs_value(t, e, k);
-    if (bad) v = 0.0f;
-    obs[(size_t)env * D + k] = v;
-  }
-  bool truncated = false;
-  if (lane == 0) {
-    float r = rew;
-    reward[env] = r;
-    // episode statistics and time limit (include/locosim.h): length and return of the running episode, the two limits,
-    // bit 1 of the done byte (absorbing wins), the finished episode's numbers
-    int4 es = st.ep[env];
-    es.x += 1; es.y = __float_as_int(__int_as_float(es.y) + r);
-    truncated = st.max_episode_steps > 0 && es.x >= st.max_episode_steps;
-    if (st.end_of_trajectory) {
-      // one (clamped) advance of the cursor per step: the tracking reward above has made it already
-      const int cur = st.cursor[env];
-      int sp = cur % t.traj_len;
-      if (t.reward_type != LS_REWARD_TRACKING && sp + 1 < t.traj_len) { sp += 1; st.cursor[env] = cur + 1; }
-      truncated |= sp == t.traj_len - 1;
-    }
-    truncated = truncated && !is_done;
-    done[env] = is_done ? 1 : (truncated ? 2 : 0);
-    if (is_done || truncated) { es.z = es.x; es.w = es.y; }
-    st.ep[env] = es;
-    int* cnt = st.counters + (size_t)env * 8;
-    cnt[0] += 1; cnt[2] = e.iter_sum; cnt[3] = e.ncon;
-    if (bad) cnt[4] += 1;
-    {
-      int key = e.iter_sum;
-      const int mpr_w = (key_mode >> 8) & 255;           // weight of one MPR run in Newton-iteration units
-      key_mode &= 255;
-      if (key_mode == 1) key = (cnt[5] + e.iter_sum + 1) >> 1;
-      else if (key_mode == 2) key = e.solver_iter * 8;
-      else if (key_mode == 3) key = e.iter_sum + (e.nefc >> 1) + mpr_w * min(e.mpr_calls, 64);
-      else if (key_mode == 4) key = (3 * cnt[5] + e.iter_sum + 2) >> 2;
-      else if (key_mode == 5) key = e.iter_sum + 4 * e.solver_iter;
-      else if (key_mode == 6) key = e.iter_sum + e.nefc;
-      else if (key_mode == 7) key = e.iter_sum + 4 * e.solver_iter + (e.nefc >> 1);
-      cnt[5] = key;
-    } cnt[6] = max(cnt[6], e.ncon); cnt[7] = max(cnt[7], e.nefc);
-  }
-
-  // ---- auto-reset (reset_env is a whole-warp call: lane 0's verdict on the time limit goes to every lane first) ----
-  truncated = __shfl_sync(0xffffffffu, (int)truncated, 0) != 0;
-  if ((is_done || truncated) && (auto_reset || bad)) {
-    const int key_reset = (key_mode_in >> 16) ? (key_mode_in >> 16) - 1 : -1;
-    int ep = st.episode[env];
-    int tr, sp;
-    draw_reset(seed, env_off + env, ep, t.n_traj, t.traj_len, &tr, &sp);
-    __syncwarp();
-    reset_env(ms, t, e, tr, sp, t.rot[0] >= 0 ? draw_rot_angle(seed, env_off + env, ep) : 0.0f);
-    if (lane == 0) {
-      const int prow = draw_pool_row(seed, env_off + env, ep, st.pool_K);
-      st.episode[env] = ep + 1; st.counters[(size_t)env * 8 + 1] += 1;
-      if (key_reset >= 0) st.counters[(size_t)env * 8 + 5] = key_reset;   // regrouping key of a fresh episode (the finished one's says nothing)
-      st.dr_row[env] = prow;
-      st.cursor[env] = tr * t.traj_len + sp;
-      *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
-      e.prm = st.pool + (size_t)prow * m.pool_P;      // the next episode's model (LS_OBS_PARAM entries of next_obs)
-    }
-    __syncwarp();
-    for (int k = lane; k < t.n_goal; k += 32) st.goal[(size_t)env * 4 + k] = e.goal[k];
-  }
-  if (next_obs) for (int k = lane; k < D; k += 32) next_obs[(size_t)env * D + k] = obs_value(t, e, k);
-
-  // ---- store state ----
-  for (int i = lane; i < nv; i += 32) {
-    st.qpos[(size_t)env * nv + i] = e.qpos[i];
-    st.qvel[(size_t)env * nv + i] = e.qvel[i];
-    st.ws[(size_t)env * nv + i] = e.qacc_ws[i];
-  }
+  const bool reset = step_epilogue<C>(ms, t, st, e, env, rew, obs, reward, done, next_obs, auto_reset, seed, env_off,
+                                      key_mode_in);
   __threadfence();
   __syncwarp();
   if (lane == 0) {
     // into chunk 0 of the next step
-    int key = launch_key(t, e, k0, k1, iter0, mpr0, key_mode_in);
-    if ((is_done || truncated) && (auto_reset || bad) && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
+    if (reset && (key_mode_in >> 16)) key = (key_mode_in >> 16) - 1;
     persist_publish(q, par, q.nch, env, n_envs, key);
   }
   PH_LAP(PH_EPILOGUE, t_epi);
@@ -969,25 +779,7 @@ __global__ void __launch_bounds__(512, 1) persist_kernel(int ms, DevTask t, Solv
   __shared__ int s_env[16], s_n, s_c, s_par, s_it[2];
   __shared__ long long s_t[2];   // timeline: pop start, group start (in shared memory: nothing extra live across the body)
   const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  if (stage_bytes > 0) {
-    // the TMA-staged pair table of step_kernel, once per block for the whole step
-    unsigned char* dst = smem_raw + (size_t)wpb * sizeof(EnvS<C>);
-    const unsigned dst_a = (unsigned)__cvta_generic_to_shared(dst);
-    const unsigned bar_a = dst_a + (unsigned)stage_bytes;
-    if (threadIdx.x == 0) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"((unsigned)stage_bytes) : "memory");
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
-                   "l"(stage_src), "r"((unsigned)stage_bytes), "r"(bar_a)
-                   : "memory");
-    }
-    __syncthreads();                                    // (the barrier object is initialised before anybody polls it)
-    unsigned ok = 0;
-    while (!ok)
-      asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                   : "=r"(ok) : "r"(bar_a) : "memory");
-  }
+  stage_pair_table<C>(smem_raw, stage_src, stage_bytes);   // once per block for the whole step
   if (threadIdx.x == 0) s_par = __ldcg(&q.seq[0]) & 1;
   __syncthreads();
   for (;;) {
