@@ -162,6 +162,34 @@ int locosim_set_applied_forces(locosim_t* h, float* d_xfrc, float* d_qfrc);
 #define LS_BODY_DIM 13
 int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body);
 
+/* Contact outputs, MuJoCo's contact forces summed per body (what a loco-mujoco user computes with mj_contactForce over
+ * env._data.contact): a caller-owned DEVICE buffer d_contact, fp32 [n_envs, nbody, LS_CONTACT_DIM]. Rows are the compiled
+ * model's body indices, as for xfrc_applied and the body outputs. Per body 6 values, the wrench exerted ON the body BY all of
+ * its contacts:
+ *   force (3)  world coordinates
+ *   torque (3) world coordinates, about the body-frame origin xpos (the point of the body outputs' linear velocity). NOT the
+ *              centre of mass, and NOT the subtree_com convention of MuJoCo's cfrc_ext.
+ * Per contact, f = the contact-frame force of mj_contactForce (elliptic cones: the dim constraint forces; pyramidal cones:
+ * mju_decodePyramid; dim 1, 3, 4 and 6), and with the frame rows n, t1, t2 (n points from geom1 to geom2):
+ *   F = f0 n + f1 t1 + f2 t2,  T = f3 n + f4 t1 + f5 t2 (the components past dim are zero).
+ * The contact adds +F and (pos - xpos[b2]) x F + T to geom2's body b2, and -F and -((pos - xpos[b1]) x F + T) to geom1's body
+ * b1 (the signs of mj_rnePostConstraint). A self contact therefore appears in two rows with opposite signs. Row 0 (the world)
+ * is all zeros.
+ * Time window: the MEAN over the control step's sub-steps; each sub-step contributes the contact list, xpos and constraint
+ * forces of its last dynamics evaluation (Euler: its only one; RK4: its fourth stage), the window and evaluation of the
+ * use_foot_forces observation. This differs from MuJoCo's mjData after mj_step, which holds the last sub-step only. Contacts
+ * dropped by the per-env cap of the constraint set (DESIGN.md section 7) are not in the sum.
+ * Written by every locosim_step for every env it advances: the row describes the step that produced d_obs (for an env that
+ * ended and was auto-reset: its terminal step; for a non-finite env all zeros, as its observation). Not written by
+ * locosim_reset* or locosim_set_state. NULL = off = the state after locosim_create: nothing is written, and no other output
+ * changes by a bit; with the buffer registered no other output changes by a bit either. Register outside of stream capture,
+ * like locosim_set_applied_forces.
+ * CUDA graphs: the step kernels read the pointer from engine state on the device when they run, and no kernel is added. A
+ * step captured BEFORE the registration therefore writes the buffer when it is replayed after it (unlike the body outputs),
+ * and registering NULL stops a captured step writing. */
+#define LS_CONTACT_DIM 6
+int locosim_set_contact_outputs(locosim_t* h, float* d_contact);
+
 /* Replaces LocoEnv.create_dataset() (base.py:278-312 -> utils/trajectory.py:104-151) on the device: consecutive samples of
  * every trajectory of the reset table in observation layout. d_states / d_next_states fp32 [locosim_dataset_rows, obs_dim],
  * d_last fp32 [locosim_dataset_rows] (may be NULL); absorbing is all zero in the reference and is not materialised. */

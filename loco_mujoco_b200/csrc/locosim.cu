@@ -394,6 +394,7 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int ms, DevTask t, SolverO
   if (lane == 0) {
     e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
     e.env = env;
+    e.substep = ghost ? -1 : 0;
     if (stage_bytes > 0) {
       const unsigned char* sm = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
       e.pk_tab = reinterpret_cast<const int*>(sm);
@@ -456,6 +457,7 @@ __device__ __forceinline__ void substep_body(unsigned char* smem_raw, int ms, co
   if (lane == 0) {
     e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
     e.env = env;
+    e.substep = ghost ? -1 : k0;
     if (stage_bytes > 0) {
       const unsigned char* sm = smem_raw + (size_t)(blockDim.x >> 5) * sizeof(EnvS<C>);
       e.pk_tab = reinterpret_cast<const int*>(sm);
@@ -691,6 +693,7 @@ __device__ __forceinline__ int persist_body(unsigned char* smem_raw, int ms, con
   const DevModel& m = c_models[ms];
   const int nv = m.nv, nu = m.nu;
   e.env = env;     // (every lane: a predicated store costs the persistent kernel a spill)
+  e.substep = ghost ? -1 : k0;
   if (lane == 0) {
     e.prm = st.pool + (size_t)__ldcg(&st.dr_row[env]) * m.pool_P;
     if (stage_bytes > 0) {
@@ -920,6 +923,7 @@ struct locosim_handle {
   DevModel dm;
   DevApplied applied = {nullptr, nullptr};
   DevBodyOut bodyout = {nullptr, nullptr, nullptr};
+  DevContact contact = {nullptr, 1};
   DevTask dt;
   SolverOpts so;
   EngineState st;
@@ -1220,7 +1224,8 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
   if (h->slot < 0) { locosim_destroy(h); g_create_error = "too many live locosim handles (max 16 per process)"; return 1; }
   if (cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot) != cudaSuccess ||
-      cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot) != cudaSuccess) {
+      cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot) != cudaSuccess) {
     g_create_error = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); return 1;
   }
   bind_task(h->dt, h->ht, h->hm.nu, h->d_tints, h->d_treals);
@@ -1309,6 +1314,16 @@ int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body) {
   h->bodyout.body = d_body; h->bodyout.next_body = d_next_body;
   // (a __constant__ table of its own in both translation units, like the applied forces)
   CK(cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot));
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  return 0;
+}
+int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {
+  CK(cudaSetDevice(h->device));
+  h->contact.wrench = d_contact;
+  h->contact.n_substeps = h->dt.n_substeps;
+  // (a __constant__ table of its own in both translation units; the step kernels read it when they run, so a step captured
+  // in a CUDA graph before this call writes the buffer at its next replay)
+  CK(cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot));
   if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   return 0;
 }

@@ -17,7 +17,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#include "../../include/locosim.h"            // (LS_BODY_DIM)
+#include "../../include/locosim.h"            // (LS_BODY_DIM, LS_CONTACT_DIM)
 #include "../../include/locosim_modelpack.h"
 #include "../../include/locosim_task.h"
 
@@ -38,6 +38,7 @@ struct alignas(16) float4 { float x, y, z, w; };
 #define BLOCK_ANY(flag, pred) (pred)
 #define BLOCK_SYNC(flag) ((void)0)
 #define LS_LDG(p) (*(p))
+#define LS_LDCG(p) (*(p))
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 #else
 #define LS_DEV __device__ __forceinline__
@@ -51,6 +52,7 @@ static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 #define LS_FFS(x) __ffs((int)(x))
 #define LS_CLZ(x) __clz((int)(x))
 #define LS_LDG(p) __ldg(p)           // read-only path (caller-owned inputs that no warp writes before its last read)
+#define LS_LDCG(p) __ldcg(p)         // past L1 (rows another SM of the same launch may have written)
 // OR-reduction that doubles as a barrier: keeps warps in the same solver iteration (flag = 0: plain predicate).
 // flag = number of consecutive warps that iterate in lock-step (a GROUP): flag >= warps per block -> the whole block
 // (__syncthreads_or); smaller groups use one named barrier each (barrier.red with a thread count), so a group only waits
@@ -134,6 +136,14 @@ struct DevBodyOut {
   int* reset_mark;
 };
 
+// contact outputs of a handle (locosim_set_contact_outputs): caller-owned [N, nb, LS_CONTACT_DIM] per-body contact wrenches
+// (force, torque about xpos; world frame), row EnvS::env, the mean over the n_substeps sub-steps of a control step (the
+// task's); NULL = not written
+struct DevContact {
+  float* wrench;
+  int n_substeps;
+};
+
 struct DevTask {
   int obs_dim, n_done, reward_type, n_substeps, n_traj, traj_len, n_goal, recenter0, recenter1, ri[4], use_absorbing;
   int n_grf;                      // foot-force groups (use_foot_forces), 0 = off
@@ -152,11 +162,13 @@ struct DevTask {
 static DevModel c_models[LS_MAX_SLOTS];
 static DevApplied c_applied[LS_MAX_SLOTS];
 static DevBodyOut c_bodyout[LS_MAX_SLOTS];
+static DevContact c_contact[LS_MAX_SLOTS];
 static int c_debug = 0;
 #else
 __constant__ DevModel c_models[LS_MAX_SLOTS];
 __constant__ DevApplied c_applied[LS_MAX_SLOTS];   // (a table of its own: DevModel's layout, and the code reading it, stay as they are)
 __constant__ DevBodyOut c_bodyout[LS_MAX_SLOTS];  // (likewise)
+__constant__ DevContact c_contact[LS_MAX_SLOTS];  // (likewise)
 __constant__ int c_debug;      // diagnostic switches (LOCOSIM_DEBUG): 1 skip MPR, 2 skip the OBB filter, 4 drop convex pairs,
                                // 8 count MPR runs / support calls (locosim_debug_counters), 16 no separating-direction cache
 __device__ unsigned long long g_dbg[8];      // (LOCOSIM_DEBUG & 8) MPR statistics: calls, support pairs, hits, cap exits
@@ -209,7 +221,9 @@ struct alignas(16) EnvS {
   // kinematics that stays alive through collision / constraint assembly
   float xpos[NB][3], xquat[NB][4], xmat[NB][9];
   float gxpos[NG][3];
-  float com[4];
+  float com[3];
+  int substep;             // contact outputs: index within the control step of the next sub-step (-1: a warp that shadows
+                           // another env, which writes no outputs); set by the kernels, advanced by contact_wrench
   float cdof[NV][6];
   float M[NV][NVP], H[NV][NVP];                              // H: chol(M) during smooth_forces, then the Newton Hessian factor
   // contacts
@@ -2718,9 +2732,90 @@ LS_FN void rk4_step(const int ms, EnvS<C>& e, const SolverOpts so) {
   SYNC();
 }
 
+// mj_contactForce: the contact-frame force of contact ci (normal, tangent 1, tangent 2, torsion, rolling 1, rolling 2; zeros
+// past its dim) from the constraint forces of the last forward evaluation
+template <class C>
+LS_DEV void contact_frame_force(const EnvS<C>& e, const int ci, float* f) {
+  const int r0 = e.nunit + e.con_row[ci], dim = e.con_dim[ci];
+#pragma unroll
+  for (int j = 0; j < 6; j++) f[j] = 0;
+  if (dim == 1) f[0] = e.r_force[r0];
+  else if (C::CONE == 1) {
+#pragma unroll
+    for (int j = 0; j < 6; j++) if (j < dim) f[j] = e.r_force[r0 + j];
+  } else {
+    // mju_decodePyramid: normal = sum of the edge forces, component i = (f_2(i-1) - f_2(i-1)+1) * mu_(i-1)
+    const int ne = 2 * (dim - 1);
+    NOUNROLL for (int j = 0; j < ne; j++) f[0] += e.r_force[r0 + j];
+#pragma unroll
+    for (int j = 1; j < 6; j++)
+      if (j < dim) f[j] = (e.r_force[r0 + 2 * (j - 1)] - e.r_force[r0 + 2 * (j - 1) + 1]) * e.con_fri[ci][j - 1];
+  }
+}
+
+// contact outputs (locosim_set_contact_outputs): per body the wrench its contacts of this sub-step's last forward evaluation
+// exert on it (force, and torque about xpos, world frame), accumulated into the env's row of the caller's buffer as the mean
+// over the control step's n_sub sub-steps: global sub-step k = 0 writes, later ones add, k = n_sub - 1 scales by 1 / n_sub.
+// The buffer is the only carry, so the sub-step and persistent kernels need no field of their own. One lane per body, each
+// scanning the contact list in list order: the same summation order in every kernel, and no atomics. The row is read past L1
+// (the persistent kernel: another SM may have written it in an earlier chunk of the step).
+// After the last sub-step the row of a non-finite env is zeroed, as its observation is (the epilogue's test on the same
+// state; made here rather than in the epilogue, where it costs every step kernel spills whether or not anything is
+// registered). The sub-step index lives in EnvS::substep, not in an argument: a value live across the sub-step changes
+// the step kernels' register allocation and stack frames whether or not anything is registered.
+template <class C>
+LS_FN void contact_wrench(const int ms, EnvS<C>& e) {
+  static_assert(C::NB <= 32, "contact_wrench: one lane per body");
+  const int k = e.substep;
+  if (k < 0) return;
+  const DevModel& m = c_models[ms];
+  const int n_sub = c_contact[ms].n_substeps;
+  float* row = c_contact[ms].wrench + (size_t)e.env * m.nb * LS_CONTACT_DIM;
+  const int ncon = e.ncon;
+  bool bad = false;
+  if (k == n_sub - 1) {
+    PAR_FOR(i, m.nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+#ifndef LS_EMULATE
+    bad = __any_sync(0xffffffffu, bad);
+#endif
+  }
+  PAR_FOR(b, m.nb) {
+    float w[6] = {0, 0, 0, 0, 0, 0};
+    if (b > 0) {                                   // (the world row stays exact zeros)
+      NOUNROLL for (int ci = 0; ci < ncon; ci++) {
+        const int b1 = m.geom_bodyid[e.con_g1[ci]], b2 = m.geom_bodyid[e.con_g2[ci]];
+        if (b != b1 && b != b2) continue;
+        float f[6];
+        contact_frame_force(e, ci, f);
+        const float* fr = e.con_frame[ci];
+        float F[3], T[3], rxF[3];
+        for (int c = 0; c < 3; c++) {
+          F[c] = f[0] * fr[c] + f[1] * fr[3 + c] + f[2] * fr[6 + c];
+          T[c] = f[3] * fr[c] + f[4] * fr[3 + c] + f[5] * fr[6 + c];
+        }
+        const float r[3] = {e.con_pos[ci][0] - e.xpos[b][0], e.con_pos[ci][1] - e.xpos[b][1], e.con_pos[ci][2] - e.xpos[b][2]};
+        cross3(rxF, r, F);
+        // the frame normal points from geom1 to geom2: +wrench on geom2's body, - on geom1's (mj_rnePostConstraint)
+        const float s = b == b2 ? 1.0f : -1.0f;
+        for (int c = 0; c < 3; c++) { w[c] += s * F[c]; w[3 + c] += s * (rxF[c] + T[c]); }
+      }
+    }
+    float* dst = row + b * LS_CONTACT_DIM;
+    for (int c = 0; c < LS_CONTACT_DIM; c++) {
+      float v = k == 0 ? w[c] : LS_LDCG(dst + c) + w[c];
+      if (k == n_sub - 1) v = bad ? 0.0f : v * (1.0f / (float)n_sub);
+      dst[c] = v;
+    }
+  }
+  SYNC();
+  LANE0 e.substep = k + 1;
+  SYNC();
+}
+
 // use_foot_forces (base.py:623-631,656-679 -> mushroom _get_collision_force -> mj_contactForce): per foot group the
 // contact-frame force (normal, tangent 1, tangent 2) of the FIRST contact between the floor and a geom of the group, in
-// contact-list order, from the constraint forces of the sub-step's (last) forward evaluation; summed over sub-steps.
+// contact-list order, from the constraint forces of the sub-step's (last) forward evaluation; summed over sub-steps. Then
+// the contact outputs of the sub-step, while registered.
 template <class C>
 LS_FN void contact_forces(const int ms, EnvS<C>& e, const int* grf_group, int n_grf) {
   const int nunit = e.nunit, ncon = e.ncon;
@@ -2737,7 +2832,7 @@ LS_FN void contact_forces(const int ms, EnvS<C>& e, const int* grf_group, int n_
       if ((ga == LS_GRF_FLOOR && gb == k) || (gb == LS_GRF_FLOOR && ga == k)) first = ci;
     }
 #else
-  if (lane < ncon) { ga = grf_group[e.con_g1[lane]]; gb = grf_group[e.con_g2[lane]]; }
+  if (n_grf > 0 && lane < ncon) { ga = grf_group[e.con_g1[lane]]; gb = grf_group[e.con_g2[lane]]; }
   for (int k = 0; k < n_grf; k++) {
     const bool hit = (ga == LS_GRF_FLOOR && gb == k) || (gb == LS_GRF_FLOOR && ga == k);
     const unsigned mask = __ballot_sync(0xffffffffu, hit);
@@ -2745,22 +2840,13 @@ LS_FN void contact_forces(const int ms, EnvS<C>& e, const int* grf_group, int n_
 #endif
     if (first >= ncon) continue;
     LANE0 {
-      const int ci = first, r0 = nunit + e.con_row[ci], dim = e.con_dim[ci];
-      float f0 = 0, f1 = 0, f2 = 0;
-      if (dim == 1) f0 = e.r_force[r0];
-      else if (C::CONE == 1) {
-        f0 = e.r_force[r0]; f1 = e.r_force[r0 + 1]; f2 = e.r_force[r0 + 2];
-      } else {
-        // mju_decodePyramid: normal = sum of the edge forces, tangent_i = (f_2i - f_2i+1) * mu_i
-        const int ne = 2 * (dim - 1);
-        NOUNROLL for (int j = 0; j < ne; j++) f0 += e.r_force[r0 + j];
-        f1 = (e.r_force[r0] - e.r_force[r0 + 1]) * e.con_fri[ci][0];
-        if (dim > 2) f2 = (e.r_force[r0 + 2] - e.r_force[r0 + 3]) * e.con_fri[ci][1];
-      }
-      e.grf[3 * k] += f0; e.grf[3 * k + 1] += f1; e.grf[3 * k + 2] += f2;
+      float f[6];
+      contact_frame_force(e, first, f);
+      e.grf[3 * k] += f[0]; e.grf[3 * k + 1] += f[1]; e.grf[3 * k + 2] += f[2];
     }
   }
   SYNC();
+  if (c_contact[ms].wrench) contact_wrench(ms, e);
 }
 
 template <class C>
@@ -2771,7 +2857,9 @@ LS_FN void physics_substeps(const int ms, EnvS<C>& e, const SolverOpts so, int n
     forward(ms, e, so);
     PH_T0(t);
     if constexpr (C::RK4 == 1) rk4_step(ms, e, so); else euler_step(ms, e);
-    if (n_grf > 0) contact_forces(ms, e, grf_group, n_grf);
+    // (the contact outputs are written from contact_forces' call rather than a call of their own: another call site here
+    //  changes the step kernels' register allocation and spills whether or not anything is registered)
+    if (n_grf > 0 || c_contact[ms].wrench) contact_forces(ms, e, grf_group, n_grf);
     PH_LAP(PH_INTEGRATOR, t);
     PH_LAP(PH_SUBSTEP, t_sub);
     PH_CNT(PH_SUBSTEPS, 1);

@@ -12,6 +12,7 @@ struct EmuBase {
   HostModel hm;
   DevModel m;
   DevApplied ap = {nullptr, nullptr};
+  DevContact cw = {nullptr, 1};
   SolverOpts so;
   std::vector<int> grf_group; int n_grf = 0;
   virtual ~EmuBase() {}
@@ -37,7 +38,8 @@ struct EmuT : EmuBase {
   }
   void step(const double* ctrl, int nsub) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
-    c_models[0] = m; c_applied[0] = ap;
+    c_models[0] = m; c_applied[0] = ap; c_contact[0] = cw; c_contact[0].n_substeps = nsub;
+    e.substep = 0;
     physics_substeps(0, e, so, nsub, grf_group.data(), n_grf);
   }
   void fwd(const double* ctrl) override {
@@ -132,6 +134,9 @@ void emu_set_ws(EmuBase* s, const double* w) { s->set_ws(w); }
 void emu_set_applied(EmuBase* s, float* xfrc, float* qfrc) { s->ap.xfrc = xfrc; s->ap.qfrc = qfrc; }
 // body outputs of the emulated env's current state (locosim_set_body_outputs): fp32 [nb, LS_BODY_DIM] into `out`
 void emu_body_outputs(EmuBase* s, float* out) { s->body(out); }
+// contact outputs of the emulated env (locosim_set_contact_outputs; row 0 of the engine's layout: fp32 [nb, LS_CONTACT_DIM], or
+// NULL): every later emu_step(ctrl, nsub) runs as one control step of nsub sub-steps and leaves their mean wrench there
+void emu_set_contact(EmuBase* s, float* wrench) { s->cw.wrench = wrench; }
 long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, 0}; return v[k]; }
 long emu_ls_evals() { return g_ls_evals; }
 long emu_ls_searches() { return g_ls_searches; }

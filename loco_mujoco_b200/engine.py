@@ -84,6 +84,8 @@ def load_library():
     lib.locosim_set_applied_forces.argtypes = [vp, vp, vp]
     lib.locosim_set_body_outputs.restype = ip
     lib.locosim_set_body_outputs.argtypes = [vp, vp, vp]
+    lib.locosim_set_contact_outputs.restype = ip
+    lib.locosim_set_contact_outputs.argtypes = [vp, vp]
     _LIB = lib
     return lib
 
@@ -96,11 +98,13 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_set_reset_rotation", "locosim_get_cursor", "locosim_dataset_rows", "locosim_create_dataset",
                     "locosim_debug_counters", "locosim_set_timeline", "locosim_set_time_limit",
                     "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
-                    "locosim_set_body_outputs"]
+                    "locosim_set_body_outputs", "locosim_set_contact_outputs"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
 BODY_DIM = 13
+# values per body row of the contact outputs (include/locosim.h LS_CONTACT_DIM): force (3), torque about xpos (3), world frame
+CONTACT_DIM = 6
 
 # bits of the done byte of a step (include/locosim.h)
 DONE_ABSORBING, DONE_TRUNCATED = 1, 2
@@ -172,6 +176,7 @@ class CudaEngine:
         self.nbody = self.lib.locosim_nbody(h)
         self._applied = (None, None)      # the registered applied-force tensors (kept alive while registered)
         self._body_out = (None, None)     # the registered body-output tensors (likewise)
+        self._contact_out = None          # the registered contact-output tensor (likewise)
         # obs / reward / done of a step live in ONE device allocation (three views), so that a consumer on the host can
         # fetch the whole step result with a single D2H copy of `packed_out`
         N, D = int(n_envs), self.obs_dim
@@ -300,6 +305,22 @@ class CudaEngine:
         self._check(self.lib.locosim_set_body_outputs(self.h, _ptr(body), _ptr(next_body)))
         self._body_out = (body, next_body)
         self.kernels_per_step = self.lib.locosim_kernels_per_step(self.h)     # (+1 while registered: body_kernel)
+
+    def set_contact_outputs(self, contact=None):
+        """Register the contact outputs of include/locosim.h (MuJoCo's mj_contactForce summed per body): `contact` float32
+        cuda [n_envs, nbody, CONTACT_DIM], or None to turn the feature off. Every step writes, per body, the world-frame force
+        and torque about the body-frame origin that the body's contacts exert on it, averaged over the step's sub-steps
+        (zeros for a non-finite env). reset() and set_state() leave it alone. The engine keeps a reference to it. Register
+        outside of CUDA-graph capture; a step captured earlier writes the buffer registered when it is replayed."""
+        t = self.torch
+        if contact is not None:
+            shape = (self.n_envs, self.nbody, CONTACT_DIM)
+            if contact.dtype != t.float32 or not contact.is_contiguous() or contact.device != self.device:
+                raise ValueError("contact must be a contiguous float32 tensor on %s" % self.device)
+            if tuple(contact.shape) != shape:
+                raise ValueError("contact shape %s != %s" % (tuple(contact.shape), shape))
+        self._check(self.lib.locosim_set_contact_outputs(self.h, _ptr(contact)))
+        self._contact_out = contact
 
     def episode_stats(self):
         """(length int32, return float32, last_length, last_return), each [n_envs]: the running episode's control steps and

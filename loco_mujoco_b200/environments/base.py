@@ -241,6 +241,8 @@ class LocoEnv:
         # body outputs (body_state / next_body_state below): allocated and registered with the engine on first access
         self._body_state = None
         self._next_body_state = None
+        # contact outputs (contact_wrench below): allocated and registered with the engine on first access
+        self._contact_wrench = None
         self._engine = None
         self._obs = None
 
@@ -435,13 +437,16 @@ class LocoEnv:
                 self._engine.set_applied_forces(self._xfrc_applied, self._qfrc_applied)
             if self._body_state is not None:
                 self._engine.set_body_outputs(self._body_state, self._next_body_state)
+            if self._contact_wrench is not None:
+                self._engine.set_contact_outputs(self._contact_wrench)
         return self._engine
 
     # ---------------------------------------------------------------------------------------------------
     # applied forces (MuJoCo's mjData.xfrc_applied / qfrc_applied, include/locosim.h locosim_set_applied_forces)
     # ---------------------------------------------------------------------------------------------------
     def body_index(self, name):
-        """Row of body `name` in `xfrc_applied`, `body_state` and `next_body_state` (an index of the compiled model).
+        """Row of body `name` in `xfrc_applied`, `body_state`, `next_body_state` and `contact_wrench` (an index of the compiled
+        model).
         ValueError for an unknown name and for a body that fuse_static merged into its parent; the message then names the
         parent."""
         return self._model.body_index(name)
@@ -508,6 +513,32 @@ class LocoEnv:
         self._body_state = torch.zeros(shape, dtype=torch.float32, device=eng.device)
         self._next_body_state = torch.zeros(shape, dtype=torch.float32, device=eng.device)
         eng.set_body_outputs(self._body_state, self._next_body_state)
+
+    # ---------------------------------------------------------------------------------------------------
+    # contact outputs (MuJoCo's mj_contactForce summed per body, include/locosim.h locosim_set_contact_outputs)
+    # ---------------------------------------------------------------------------------------------------
+    @property
+    def contact_wrench(self):
+        """float32 torch tensor [num_envs, nbody, CONTACT_DIM = 6] on the env's device, rewritten by every step: per body (row
+        `body_index(name)`) the force (3) and the torque (3) that all of the body's contacts exert on it, in world
+        coordinates, the torque about the body-frame origin xpos (the point of `body_state`'s linear velocity; not the centre
+        of mass, and not the subtree_com convention of MuJoCo's cfrc_ext). Each contact's force is mj_contactForce's (every
+        component of its condim, torsional and rolling included), turned into the world frame; it acts with + on geom2's
+        body and with - on geom1's, so a self contact appears in two rows with opposite signs. Row 0 (the world) is zero.
+        The values are the MEAN over the step's sub-steps (each sub-step's last dynamics evaluation, the window of the
+        foot-force observation), not MuJoCo's last sub-step; contacts past the engine's per-env cap are not in the sum. It
+        describes the step that produced the observation: for an env that ended, its terminal step; for an env whose state
+        became non-finite, zeros. reset() does not write it. Allocated zeroed and registered on first access: an env that
+        never touches it computes nothing extra. A step captured in a CUDA graph before the first access writes it from
+        the next replay on."""
+        if self._contact_wrench is None:
+            import torch
+            from ..engine import CONTACT_DIM
+            eng = self._get_engine()
+            t = torch.zeros((self.num_envs, self._model.nbody, CONTACT_DIM), dtype=torch.float32, device=eng.device)
+            eng.set_contact_outputs(t)
+            self._contact_wrench = t
+        return self._contact_wrench
 
     # ---------------------------------------------------------------------------------------------------
     # the hot path

@@ -308,6 +308,13 @@ class HumanoidTorque4AgesAll:
     body_state = property(_no_body_outputs)
     next_body_state = property(_no_body_outputs)
 
+    # ---- contact outputs: likewise ----
+    def _no_contact_outputs(self, *args):
+        raise NotImplementedError("contact outputs (contact_wrench) are not available for HumanoidTorque4Ages mode 'all': "
+                                  "use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
+
+    contact_wrench = property(_no_contact_outputs)
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch
