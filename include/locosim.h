@@ -190,6 +190,28 @@ int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body);
 #define LS_CONTACT_DIM 6
 int locosim_set_contact_outputs(locosim_t* h, float* d_contact);
 
+/* Per-dof outputs, MuJoCo's mjData.qfrc_actuator / qfrc_constraint / qacc (what a loco-mujoco user reads from env._data for
+ * torque, joint-limit and acceleration penalties): a caller-owned DEVICE buffer d_dof, fp32 [n_envs, nq, LS_DOF_DIM]. Every
+ * in-scope model has nq == nv (hinge and slide joints only), so rows are dof indices: the qvel layout of locosim_get_state
+ * and of qfrc_applied. Per dof 3 values:
+ *   0 qfrc_actuator    sum over the actuators on the dof of gear * force, the force of mj_fwdActuation: ctrl clamped to
+ *                      ctrlrange, gain * ctrl + bias0 + bias1 * qpos + bias2 * qvel at the evaluation's state, clamped to
+ *                      forcerange
+ *   1 qfrc_constraint  J^T efc_force at the solver's final qacc, as mj_fwdConstraint leaves it
+ *   2 qacc             the constrained acceleration of mj_forward. For the Euler integrator this is NOT the solve with
+ *                      implicit joint damping that the integrator advances with (which MuJoCo also keeps out of d->qacc).
+ * Time window: the MEAN over the control step's sub-steps; each sub-step contributes its last dynamics evaluation (Euler: its
+ * only one; RK4: its fourth stage), the window of the contact outputs. This differs from MuJoCo's mjData after mj_step, which
+ * holds the last sub-step only, evaluated at that sub-step's START state (RK4: its first stage).
+ * Written by every locosim_step for every env it advances: the row describes the step that produced d_obs (for an env that
+ * ended and was auto-reset: its terminal step; for a non-finite env all zeros, as its observation). Not written by
+ * locosim_reset* or locosim_set_state. NULL = off = the state after locosim_create: nothing is written, and no other output
+ * changes by a bit; with the buffer registered no other output changes by a bit either. Register outside of stream capture.
+ * CUDA graphs: as for the contact outputs, the step kernels read the pointer from engine state on the device when they run
+ * and no kernel is added, so a step captured BEFORE the registration writes the buffer when it is replayed after it. */
+#define LS_DOF_DIM 3
+int locosim_set_dof_outputs(locosim_t* h, float* d_dof);
+
 /* Replaces LocoEnv.create_dataset() (base.py:278-312 -> utils/trajectory.py:104-151) on the device: consecutive samples of
  * every trajectory of the reset table in observation layout. d_states / d_next_states fp32 [locosim_dataset_rows, obs_dim],
  * d_last fp32 [locosim_dataset_rows] (may be NULL); absorbing is all zero in the reference and is not materialised. */

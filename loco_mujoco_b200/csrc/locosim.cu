@@ -924,6 +924,8 @@ struct locosim_handle {
   DevApplied applied = {nullptr, nullptr};
   DevBodyOut bodyout = {nullptr, nullptr, nullptr};
   DevContact contact = {nullptr, 1};
+  DevDof dof = {nullptr, 1};
+  float* dof_act = nullptr;          // the dof outputs' actuator-force scratch [n_envs, nu] (c_dof_act)
   DevTask dt;
   SolverOpts so;
   EngineState st;
@@ -1225,7 +1227,9 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
   if (cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot) != cudaSuccess ||
-      cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot) != cudaSuccess) {
+      cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_dof_act, &h->dof_act, sizeof(float*), sizeof(float*) * h->slot) != cudaSuccess) {
     g_create_error = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); return 1;
   }
   bind_task(h->dt, h->ht, h->hm.nu, h->d_tints, h->d_treals);
@@ -1262,6 +1266,7 @@ void locosim_destroy(locosim_t* h) {
   cudaFree(h->split.carry); cudaFree(h->split.bcount); cudaFree(h->split.benv); cudaFree(h->split.seq);
   cudaFree(h->pq.carry); cudaFree(h->pq.cnt); cudaFree(h->pq.tot); cudaFree(h->pq.benv); cudaFree(h->pq.seq);
   cudaFree(h->bodyout.reset_mark);
+  cudaFree(h->dof_act);
   delete h;
 }
 
@@ -1324,6 +1329,20 @@ int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {
   // (a __constant__ table of its own in both translation units; the step kernels read it when they run, so a step captured
   // in a CUDA graph before this call writes the buffer at its next replay)
   CK(cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot));
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  return 0;
+}
+int locosim_set_dof_outputs(locosim_t* h, float* d_dof) {
+  CK(cudaSetDevice(h->device));
+  // the actuator-force scratch [n_envs, nu] lives as long as the handle once the outputs were first registered
+  if (d_dof && !h->dof_act) {
+    CK(cudaMalloc(&h->dof_act, sizeof(float) * (size_t)h->n_envs * (h->hm.nu > 0 ? h->hm.nu : 1)));
+    CK(cudaMemcpyToSymbol(c_dof_act, &h->dof_act, sizeof(float*), sizeof(float*) * h->slot));
+  }
+  h->dof.out = d_dof;
+  h->dof.n_substeps = h->dt.n_substeps;
+  // (__constant__ tables of their own in both translation units, read when the kernels run, as for the contact outputs)
+  CK(cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot));
   if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   return 0;
 }

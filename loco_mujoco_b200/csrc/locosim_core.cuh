@@ -144,6 +144,15 @@ struct DevContact {
   int n_substeps;
 };
 
+// per-dof outputs of a handle (locosim_set_dof_outputs): caller-owned [N, nv, LS_DOF_DIM] (qfrc_actuator, qfrc_constraint,
+// qacc), row EnvS::env, the mean over the n_substeps sub-steps of a control step; NULL = not written. The layout and size
+// of DevContact: physics_substeps tests both pointers, and with a 24-byte stride the extra address arithmetic grew the
+// CfgPyrRK4 step kernel's stack frame with nothing registered.
+struct DevDof {
+  float* out;
+  int n_substeps;
+};
+
 struct DevTask {
   int obs_dim, n_done, reward_type, n_substeps, n_traj, traj_len, n_goal, recenter0, recenter1, ri[4], use_absorbing;
   int n_grf;                      // foot-force groups (use_foot_forces), 0 = off
@@ -163,6 +172,8 @@ static DevModel c_models[LS_MAX_SLOTS];
 static DevApplied c_applied[LS_MAX_SLOTS];
 static DevBodyOut c_bodyout[LS_MAX_SLOTS];
 static DevContact c_contact[LS_MAX_SLOTS];
+static DevDof c_dof[LS_MAX_SLOTS];
+static float* c_dof_act[LS_MAX_SLOTS];
 static int c_debug = 0;
 #else
 __constant__ DevModel c_models[LS_MAX_SLOTS];
@@ -171,6 +182,11 @@ __constant__ DevBodyOut c_bodyout[LS_MAX_SLOTS];  // (likewise)
 __constant__ DevContact c_contact[LS_MAX_SLOTS];  // (likewise)
 __constant__ int c_debug;      // diagnostic switches (LOCOSIM_DEBUG): 1 skip MPR, 2 skip the OBB filter, 4 drop convex pairs,
                                // 8 count MPR runs / support calls (locosim_debug_counters), 16 no separating-direction cache
+__constant__ DevDof c_dof[LS_MAX_SLOTS];          // (a table of its own, like c_contact)
+// the dof outputs' [N, nu] scratch of the force per actuator, written by every dynamics evaluation while c_dof[ms].out is
+// registered (the actuator force is folded into qfrc_smooth, and the Euler state it was evaluated at is gone after the
+// integrator), read by dof_outputs
+__constant__ float* c_dof_act[LS_MAX_SLOTS];
 __device__ unsigned long long g_dbg[8];      // (LOCOSIM_DEBUG & 8) MPR statistics: calls, support pairs, hits, cap exits
 #endif
 
@@ -222,8 +238,9 @@ struct alignas(16) EnvS {
   float xpos[NB][3], xquat[NB][4], xmat[NB][9];
   float gxpos[NG][3];
   float com[3];
-  int substep;             // contact outputs: index within the control step of the next sub-step (-1: a warp that shadows
-                           // another env, which writes no outputs); set by the kernels, advanced by contact_wrench
+  int substep;             // contact / dof outputs: index within the control step of the next sub-step (-1: a warp that
+                           // shadows another env, which writes no outputs); set by the kernels, advanced by contact_wrench
+                           // (or by dof_outputs when only those are registered)
   float cdof[NV][6];
   float M[NV][NVP], H[NV][NVP];                              // H: chol(M) during smooth_forces, then the Newton Hessian factor
   // contacts
@@ -1954,6 +1971,11 @@ LS_FN void smooth_forces(const int ms, EnvS<C>& e) {
     if (m.actuator_forcelimited[i]) f = fminf(m.actuator_forcerange[2 * i + 1], fmaxf(m.actuator_forcerange[2 * i], f));
     // one actuator per dof in all in-scope models -> no write conflict
     e.qfrc_smooth[d] += m.actuator_gear[i] * f;
+    // dof outputs: the force of this evaluation, for dof_outputs after the integrator (not from a warp that shadows
+    // another env: it may be a sub-step ahead of the env's own warp). The force, not gear * force: a second use of that
+    // product would cost the sum above its fused multiply-add, and change qfrc_smooth whether or not anything is registered.
+    float* const act = c_dof_act[ms];
+    if (act && e.substep >= 0) act[(size_t)e.env * m.nu + i] = f;
   }
   SYNC();
   PAR_FOR(j, EnvS<C>::NV) e.qacc_smooth[j] = j < nv ? e.qfrc_smooth[j] : 0.0f;
@@ -2812,6 +2834,45 @@ LS_FN void contact_wrench(const int ms, EnvS<C>& e) {
   SYNC();
 }
 
+// dof outputs (locosim_set_dof_outputs): per dof qfrc_actuator (summed over the dof's actuators in actuator order from the
+// scratch smooth_forces wrote), qfrc_constraint and qacc of this sub-step's last forward evaluation, accumulated into the
+// env's row of the caller's buffer as the contact outputs are: global sub-step k = 0 writes, later ones add, k = n_sub - 1
+// scales by 1 / n_sub and zeroes a non-finite env. One lane per dof, the same order in every kernel, no atomics; rows and
+// scratch are read past L1 (the persistent kernel: another SM may have written the row in an earlier chunk of the step).
+// Runs before contact_wrench and advances EnvS::substep only when contact_wrench will not.
+template <class C>
+LS_FN void dof_outputs(const int ms, EnvS<C>& e) {
+  const int k = e.substep;
+  if (k < 0) return;
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv, nu = m.nu, n_sub = c_dof[ms].n_substeps;
+  float* row = c_dof[ms].out + (size_t)e.env * nv * LS_DOF_DIM;
+  const float* act = c_dof_act[ms] + (size_t)e.env * nu;
+  bool bad = false;
+  if (k == n_sub - 1) {
+    PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+#ifndef LS_EMULATE
+    bad = __any_sync(0xffffffffu, bad);
+#endif
+  }
+  PAR_FOR(j, nv) {
+    float fa = 0;
+    NOUNROLL for (int i = 0; i < nu; i++) if (m.actuator_dof[i] == j) fa += m.actuator_gear[i] * LS_LDCG(act + i);
+    const float w[LS_DOF_DIM] = {fa, e.qfrc_constraint[j], e.qacc[j]};
+    float* dst = row + j * LS_DOF_DIM;
+    for (int c = 0; c < LS_DOF_DIM; c++) {
+      float v = k == 0 ? w[c] : LS_LDCG(dst + c) + w[c];
+      if (k == n_sub - 1) v = bad ? 0.0f : v * (1.0f / (float)n_sub);
+      dst[c] = v;
+    }
+  }
+  SYNC();
+  if (!c_contact[ms].wrench) {
+    LANE0 e.substep = k + 1;
+    SYNC();
+  }
+}
+
 // use_foot_forces (base.py:623-631,656-679 -> mushroom _get_collision_force -> mj_contactForce): per foot group the
 // contact-frame force (normal, tangent 1, tangent 2) of the FIRST contact between the floor and a geom of the group, in
 // contact-list order, from the constraint forces of the sub-step's (last) forward evaluation; summed over sub-steps. Then
@@ -2846,6 +2907,7 @@ LS_FN void contact_forces(const int ms, EnvS<C>& e, const int* grf_group, int n_
     }
   }
   SYNC();
+  if (c_dof[ms].out) dof_outputs(ms, e);
   if (c_contact[ms].wrench) contact_wrench(ms, e);
 }
 
@@ -2857,9 +2919,9 @@ LS_FN void physics_substeps(const int ms, EnvS<C>& e, const SolverOpts so, int n
     forward(ms, e, so);
     PH_T0(t);
     if constexpr (C::RK4 == 1) rk4_step(ms, e, so); else euler_step(ms, e);
-    // (the contact outputs are written from contact_forces' call rather than a call of their own: another call site here
-    //  changes the step kernels' register allocation and spills whether or not anything is registered)
-    if (n_grf > 0 || c_contact[ms].wrench) contact_forces(ms, e, grf_group, n_grf);
+    // (the contact and dof outputs are written from contact_forces' call rather than calls of their own: another call site
+    //  here changes the step kernels' register allocation and spills whether or not anything is registered)
+    if (n_grf > 0 || c_contact[ms].wrench || c_dof[ms].out) contact_forces(ms, e, grf_group, n_grf);
     PH_LAP(PH_INTEGRATOR, t);
     PH_LAP(PH_SUBSTEP, t_sub);
     PH_CNT(PH_SUBSTEPS, 1);

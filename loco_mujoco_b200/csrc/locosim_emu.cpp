@@ -13,6 +13,8 @@ struct EmuBase {
   DevModel m;
   DevApplied ap = {nullptr, nullptr};
   DevContact cw = {nullptr, 1};
+  DevDof dof = {nullptr, 1};
+  std::vector<float> act;            // the dof outputs' actuator-force scratch (row 0 of the engine's [N, nu])
   SolverOpts so;
   std::vector<int> grf_group; int n_grf = 0;
   virtual ~EmuBase() {}
@@ -39,12 +41,13 @@ struct EmuT : EmuBase {
   void step(const double* ctrl, int nsub) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
     c_models[0] = m; c_applied[0] = ap; c_contact[0] = cw; c_contact[0].n_substeps = nsub;
+    c_dof[0] = dof; c_dof[0].n_substeps = nsub; c_dof_act[0] = dof.out ? act.data() : nullptr;
     e.substep = 0;
     physics_substeps(0, e, so, nsub, grf_group.data(), n_grf);
   }
   void fwd(const double* ctrl) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
-    c_models[0] = m; c_applied[0] = ap;
+    c_models[0] = m; c_applied[0] = ap; c_dof[0] = dof; c_dof_act[0] = dof.out ? act.data() : nullptr;
     forward(0, e, so);
   }
   void get(double* q, double* v, double* qacc, double* ws) override {
@@ -137,6 +140,12 @@ void emu_body_outputs(EmuBase* s, float* out) { s->body(out); }
 // contact outputs of the emulated env (locosim_set_contact_outputs; row 0 of the engine's layout: fp32 [nb, LS_CONTACT_DIM], or
 // NULL): every later emu_step(ctrl, nsub) runs as one control step of nsub sub-steps and leaves their mean wrench there
 void emu_set_contact(EmuBase* s, float* wrench) { s->cw.wrench = wrench; }
+// dof outputs of the emulated env (locosim_set_dof_outputs; row 0 of the engine's layout: fp32 [nv, LS_DOF_DIM], or NULL):
+// every later emu_step(ctrl, nsub) runs as one control step of nsub sub-steps and leaves their mean there
+void emu_set_dof(EmuBase* s, float* out) {
+  s->act.assign(s->m.nu > 0 ? s->m.nu : 1, 0.0f);
+  s->dof.out = out;
+}
 long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, 0}; return v[k]; }
 long emu_ls_evals() { return g_ls_evals; }
 long emu_ls_searches() { return g_ls_searches; }

@@ -86,6 +86,8 @@ def load_library():
     lib.locosim_set_body_outputs.argtypes = [vp, vp, vp]
     lib.locosim_set_contact_outputs.restype = ip
     lib.locosim_set_contact_outputs.argtypes = [vp, vp]
+    lib.locosim_set_dof_outputs.restype = ip
+    lib.locosim_set_dof_outputs.argtypes = [vp, vp]
     _LIB = lib
     return lib
 
@@ -98,13 +100,15 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_set_reset_rotation", "locosim_get_cursor", "locosim_dataset_rows", "locosim_create_dataset",
                     "locosim_debug_counters", "locosim_set_timeline", "locosim_set_time_limit",
                     "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
-                    "locosim_set_body_outputs", "locosim_set_contact_outputs"]
+                    "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
 BODY_DIM = 13
 # values per body row of the contact outputs (include/locosim.h LS_CONTACT_DIM): force (3), torque about xpos (3), world frame
 CONTACT_DIM = 6
+# values per dof row of the dof outputs (include/locosim.h LS_DOF_DIM): qfrc_actuator, qfrc_constraint, qacc
+DOF_DIM = 3
 
 # bits of the done byte of a step (include/locosim.h)
 DONE_ABSORBING, DONE_TRUNCATED = 1, 2
@@ -177,6 +181,7 @@ class CudaEngine:
         self._applied = (None, None)      # the registered applied-force tensors (kept alive while registered)
         self._body_out = (None, None)     # the registered body-output tensors (likewise)
         self._contact_out = None          # the registered contact-output tensor (likewise)
+        self._dof_out = None              # the registered dof-output tensor (likewise)
         # obs / reward / done of a step live in ONE device allocation (three views), so that a consumer on the host can
         # fetch the whole step result with a single D2H copy of `packed_out`
         N, D = int(n_envs), self.obs_dim
@@ -321,6 +326,22 @@ class CudaEngine:
                 raise ValueError("contact shape %s != %s" % (tuple(contact.shape), shape))
         self._check(self.lib.locosim_set_contact_outputs(self.h, _ptr(contact)))
         self._contact_out = contact
+
+    def set_dof_outputs(self, dof=None):
+        """Register the dof outputs of include/locosim.h (MuJoCo's qfrc_actuator / qfrc_constraint / qacc): `dof` float32
+        cuda [n_envs, nq, DOF_DIM], or None to turn the feature off. Every step writes, per dof (the qvel layout), the actuator
+        force, the constraint force and the constrained acceleration, averaged over the step's sub-steps (zeros for a
+        non-finite env). reset() and set_state() leave it alone. The engine keeps a reference to it. Register outside of
+        CUDA-graph capture; a step captured earlier writes the buffer registered when it is replayed."""
+        t = self.torch
+        if dof is not None:
+            shape = (self.n_envs, self.nq, DOF_DIM)
+            if dof.dtype != t.float32 or not dof.is_contiguous() or dof.device != self.device:
+                raise ValueError("dof must be a contiguous float32 tensor on %s" % self.device)
+            if tuple(dof.shape) != shape:
+                raise ValueError("dof shape %s != %s" % (tuple(dof.shape), shape))
+        self._check(self.lib.locosim_set_dof_outputs(self.h, _ptr(dof)))
+        self._dof_out = dof
 
     def episode_stats(self):
         """(length int32, return float32, last_length, last_return), each [n_envs]: the running episode's control steps and

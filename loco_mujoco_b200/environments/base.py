@@ -243,6 +243,8 @@ class LocoEnv:
         self._next_body_state = None
         # contact outputs (contact_wrench below): allocated and registered with the engine on first access
         self._contact_wrench = None
+        # dof outputs (dof_outputs below): allocated and registered with the engine on first access
+        self._dof_outputs = None
         self._engine = None
         self._obs = None
 
@@ -439,6 +441,8 @@ class LocoEnv:
                 self._engine.set_body_outputs(self._body_state, self._next_body_state)
             if self._contact_wrench is not None:
                 self._engine.set_contact_outputs(self._contact_wrench)
+            if self._dof_outputs is not None:
+                self._engine.set_dof_outputs(self._dof_outputs)
         return self._engine
 
     # ---------------------------------------------------------------------------------------------------
@@ -539,6 +543,29 @@ class LocoEnv:
             eng.set_contact_outputs(t)
             self._contact_wrench = t
         return self._contact_wrench
+
+    # ---------------------------------------------------------------------------------------------------
+    # dof outputs (MuJoCo's qfrc_actuator / qfrc_constraint / qacc, include/locosim.h locosim_set_dof_outputs)
+    # ---------------------------------------------------------------------------------------------------
+    @property
+    def dof_outputs(self):
+        """float32 torch tensor [num_envs, nq, DOF_DIM = 3] on the env's device, rewritten by every step: per dof (the qvel
+        layout of the state; every model here has nq == nv) MuJoCo's qfrc_actuator (the actuators' gear * force, ctrlrange
+        and forcerange clamps applied), qfrc_constraint (J^T of the constraint forces: contacts, joint limits, friction
+        loss) and qacc (the constrained acceleration; for the Euler integrator not the implicit-damping solve it advances
+        with). The values are the MEAN over the step's sub-steps (each sub-step's last dynamics evaluation), not MuJoCo's
+        last sub-step. It describes the step that produced the observation: for an env that ended, its terminal step; for
+        an env whose state became non-finite, zeros. reset() does not write it. Allocated zeroed and registered on first
+        access: an env that never touches it computes nothing extra. A step captured in a CUDA graph before the first
+        access writes it from the next replay on."""
+        if self._dof_outputs is None:
+            import torch
+            from ..engine import DOF_DIM
+            eng = self._get_engine()
+            t = torch.zeros((self.num_envs, self._model.nq, DOF_DIM), dtype=torch.float32, device=eng.device)
+            eng.set_dof_outputs(t)
+            self._dof_outputs = t
+        return self._dof_outputs
 
     # ---------------------------------------------------------------------------------------------------
     # the hot path

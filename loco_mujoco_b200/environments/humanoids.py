@@ -315,6 +315,13 @@ class HumanoidTorque4AgesAll:
 
     contact_wrench = property(_no_contact_outputs)
 
+    # ---- dof outputs: likewise ----
+    def _no_dof_outputs(self, *args):
+        raise NotImplementedError("dof outputs (dof_outputs) are not available for HumanoidTorque4Ages mode 'all': "
+                                  "use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
+
+    dof_outputs = property(_no_dof_outputs)
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch

@@ -16,7 +16,15 @@ from ..utils.checks import check_validity_task_mode_dataset
 from ..utils.goals import GoalDirectionVelocity
 from ..utils.math import mat2angle_xy, angle2mat_xy, transform_angle_2pi, rotate_obs
 from ..utils.reward import VelocityVectorReward
-from .base import LocoEnv, ObservationType, ValidTaskConf, reference_data_root, ASSET_DIR
+from .base import LocoEnv, ObservationType, ValidTaskConf, reference_data_root, ASSET_DIR, asset_path
+
+ACTION_MODES = ("torque", "position", "position_difference")
+
+
+def _check_action_mode(action_mode):
+    if action_mode not in ACTION_MODES:
+        raise ValueError("action_mode must be one of %s, not %r" % (", ".join(map(repr, ACTION_MODES)), action_mode))
+
 
 _LEGS = ["FR", "FL", "RR", "RL"]
 _TRUNK = ["trunk_tx", "trunk_ty", "trunk_tz", "trunk_list", "trunk_tilt", "trunk_rotation"]
@@ -27,8 +35,11 @@ class UnitreeA1(LocoEnv):
 
     def __init__(self, action_mode="torque", setup_random_rot=False, default_target_velocity=0.5, camera_params=None,
                  **kwargs):
-        if action_mode != "torque":
-            raise NotImplementedError("only action_mode='torque' is built (position control models are out of scope)")
+        # "torque": twelve motors (gear 34, ctrl in [-1, 1]); "position" / "position_difference": twelve PD position
+        # actuators (kp 100, force clamped to +-33.5), whose ctrlrange is each joint's range, so the normalised action +-1
+        # is a target angle at the ends of that range (unitreeA1.py:196-218). "position_difference" is the same model and
+        # the same controller: the reference stores the mode and reads it nowhere else.
+        _check_action_mode(action_mode)
         self._action_mode = action_mode
         action_spec = self._get_action_specification()
         observation_spec = self._get_observation_specification()
@@ -41,8 +52,8 @@ class UnitreeA1(LocoEnv):
             if root is None:
                 raise FileNotFoundError("loco_mujoco model data not found (set LOCO_MUJOCO_PATH) and no compiled "
                                         "model supplied")
-            xml_handle = mjcf.XmlHandle(os.path.join(root, "environments", "data", "quadrupeds",
-                                                     "unitree_a1_torque.xml"))
+            xml = "unitree_a1_torque.xml" if action_mode == "torque" else "unitree_a1_position.xml"
+            xml_handle = mjcf.XmlHandle(os.path.join(root, "environments", "data", "quadrupeds", xml))
             # (the reference also attaches a mass-less `dir_arrow` marker body + two sites to the trunk,
             #  unitreeA1.py:755-776: visualisation only, no geoms, no inertia -> not part of the physics model)
         else:
@@ -244,7 +255,20 @@ class UnitreeA1(LocoEnv):
             mdp.load_trajectory(dict(traj_path=path, traj_dt=1 / 500.0, control_dt=mdp.dt))
         else:
             from .. import modelpack
-            asset = np.load(os.path.join(ASSET_DIR, "UnitreeA1.%s.npz" % task), allow_pickle=False)
+            action_mode = kwargs.get("action_mode", "torque")
+            if action_mode == "torque":
+                path = os.path.join(ASSET_DIR, "UnitreeA1.%s.npz" % task)
+            else:
+                _check_action_mode(action_mode)      # (an unknown mode is a ValueError, not a missing asset)
+                # both position modes share one model, UnitreeA1.<task>+position.npz; never the torque model instead
+                path = asset_path("UnitreeA1.%s+position.npz" % task)
+                if path is None:
+                    raise FileNotFoundError(
+                        "no bundled asset for UnitreeA1.%s+position (action_mode=%r): the package bundles the torque "
+                        "models; the position models are compiled from a loco_mujoco checkout (set LOCO_MUJOCO_PATH) or "
+                        "read from a directory of assets made by tools/build_assets.py (set LOCO_MUJOCO_B200_ASSET_PATH)"
+                        % (task, action_mode))
+            asset = np.load(path, allow_pickle=False)
             model = modelpack.from_npz_dict({k[6:]: asset[k] for k in asset.files if k.startswith("model_")})
             mdp = UnitreeA1(reward_type=reward_type, reward_params=reward_params, compiled_model=model, **kwargs)
             mdp.load_trajectory(dict(processed={k[5:]: asset[k] for k in asset.files if k.startswith("traj_")}))

@@ -813,8 +813,8 @@ def compile_model(handle, timestep=None, collision_mesh_max_verts=64, fuse_stati
     for sec in root.findall("actuator"):
         for ae in sec:
             a = defaults.resolve(ae, None)
-            if ae.tag not in ("motor", "general"):
-                raise NotImplementedError("actuator <%s> (in-scope torque models use <motor>)" % ae.tag)
+            if ae.tag not in ("motor", "general", "position"):
+                raise NotImplementedError("actuator <%s> (in-scope models use <motor>, <general> and <position>)" % ae.tag)
             if "joint" not in a:
                 raise NotImplementedError("only joint transmissions")
             A["name"].append(a.get("name", ""))
@@ -829,12 +829,25 @@ def compile_model(handle, timestep=None, collision_mesh_max_verts=64, fuse_stati
             A["forcelimited"].append(int(fl == "true" or (fl == "auto" and autolimits and fr[0] < fr[1])))
             A["forcerange"].append(fr)
             gp = _floats(a.get("gainprm", "1"))[0] if ae.tag == "general" else 1.0
-            A["gain"].append(gp)
             bp = np.zeros(3)
             if ae.tag == "general" and "biasprm" in a:
                 v = _floats(a["biasprm"])
                 bp[:min(3, len(v))] = v[:3]
+            if ae.tag == "position":
+                # MuJoCo 2.3.7 <position>: gainprm[0] = kp, biasprm = (0, -kp, 0), i.e. force = kp (ctrl - length)
+                gp = _floats(a.get("kp", "1"))[0]
+                bp = np.array([0.0, -gp, 0.0])
+            A["gain"].append(gp)
             A["bias"].append(bp)
+            # the engine and the oracle evaluate the bias at qpos[dof] / qvel[dof], where MuJoCo uses the actuator length
+            # gear * qpos and velocity gear * qvel of a hinge or slide joint: other cases would be computed wrongly
+            if np.any(bp[1:] != 0):
+                if J["type"][A["dof"][-1]] not in (JNT_HINGE, JNT_SLIDE):
+                    raise NotImplementedError("actuator %r: a length-dependent bias needs a hinge or slide joint"
+                                              % A["name"][-1])
+                if A["gear"][-1] != 1.0:
+                    raise NotImplementedError("actuator %r: a length-dependent bias needs gear 1, not %g"
+                                              % (A["name"][-1], A["gear"][-1]))
     m.nu = len(A["name"])
     m.actuator_names = A["name"]
     m.actuator_dof = np.array(A["dof"], dtype=np.int32)
