@@ -113,7 +113,7 @@ struct DevModel {
   const int* body_dofmask;   // [nb] bit d set if dof d is on the path root..body
   const int* dof_frow;       // [nv] index of the frictionloss row of dof d, or -1
   const int* tri_ij;         // [nv(nv+1)/2] packed (i << 8) | j of the lower triangle, row major
-  const int* pair_packed;    // [np] g1 | g2 << 12 | flags << 24 (1: plane pair, 2: convex pair) of candidate pair p
+  const int* pair_packed;    // [np] g1 | g2 << 12 | flags << 24 (1: plane pair, 2: convex pair, 4: capsule-hull test) of pair p
   const float* pair_bound;   // [np] bound of the bounding-sphere / plane mid-phase test of pair p
   // per-env parameter pool (domain randomisation): float offsets of each field inside one pool row
   int po_dof_damping, po_dof_frictionloss, po_dof_armature, po_jnt_stiffness, po_dof_invweight0, po_body_mass,
@@ -181,7 +181,8 @@ __constant__ DevApplied c_applied[LS_MAX_SLOTS];   // (a table of its own: DevMo
 __constant__ DevBodyOut c_bodyout[LS_MAX_SLOTS];  // (likewise)
 __constant__ DevContact c_contact[LS_MAX_SLOTS];  // (likewise)
 __constant__ int c_debug;      // diagnostic switches (LOCOSIM_DEBUG): 1 skip MPR, 2 skip the OBB filter, 4 drop convex pairs,
-                               // 8 count MPR runs / support calls (locosim_debug_counters), 16 no separating-direction cache
+                               // 8 count MPR runs / support calls (locosim_debug_counters), 16 no separating-direction cache,
+                               // 32 no capsule-hull test of sphere | capsule | cylinder pairs
 __constant__ DevDof c_dof[LS_MAX_SLOTS];          // (a table of its own, like c_contact)
 // the dof outputs' [N, nu] scratch of the force per actuator, written by every dynamics evaluation while c_dof[ms].out is
 // registered (the actuator force is folded into qfrc_smooth, and the Euler state it was evaluated at is gone after the
@@ -197,7 +198,12 @@ enum {
   PH_KINEMATICS, PH_COM_POS, PH_CRB_FACTOR, PH_SMOOTH_FORCES, PH_COLLISION, PH_CONVEX_QUEUE, PH_MAKE_CONSTRAINT, PH_WARMSTART,
   PH_NEWTON_WAIT, PH_NEWTON_TRIPS, PH_NEWTON_ITERS, PH_MAKE_HESSIAN, PH_CHOL_FACTOR, PH_CHOL_SOLVE, PH_LINE_SEARCH, PH_LS_EVAL,
   PH_LS_EVALS, PH_UPDATE_CONSTRAINT, PH_UPDATE_GRADIENT, PH_NEWTON_TAIL, PH_INTEGRATOR, PH_SUBSTEP, PH_SUBSTEPS, PH_PROLOGUE,
-  PH_EPILOGUE, PH_GROUPS, PH_N
+  PH_EPILOGUE, PH_GROUPS,
+  // collision() split: primitive filter rounds, primitive narrow phase + fill_contact, convex bounding-sphere loop, box (and
+  // capsule-hull) tests, the job queue's first barrier, the warp's own jobs, the barrier that waits for the block's other
+  // jobs, convex_consume; then counts of the box-test survivors and of the jobs published
+  PH_COL_PRIM_FILTER, PH_COL_PRIM_NARROW, PH_COL_SPHERES, PH_COL_OBB, PH_COL_QWAIT, PH_COL_JOBS, PH_COL_JOBS_WAIT,
+  PH_COL_CONSUME, PH_COL_NOBB, PH_COL_NJOBS, PH_N
 };
 #if defined(LOCOSIM_PHASE_CLOCK) && !defined(LS_EMULATE)
 #define LS_PH_SLOTS (256 * 16)
@@ -1225,6 +1231,59 @@ LS_DEV void geom_halfext(int type, const float* size, float mg, float* h) {
   else { h[0] = size[0] + mg; h[1] = size[1] + mg; h[2] = size[2] + mg; }
 }
 
+// Capsule-hull test of a sphere | capsule | cylinder pair (d = pos2 - pos1; m1, m2: geom frames; s1, s2: geom_size): true
+// if the geoms, each inflated by margin / 2, cannot touch. Each lies in the capsule around its axis segment (pos +- size[1]
+// along the frame's z axis; a sphere's segment is its centre) of radius size[0] (a cylinder's rim is on that capsule), so
+// axis segments further apart than the two radii plus the margin mean disjoint geoms, and MPR would report no contact.
+// The segment distance is bounded from below in fp32 without an ill-conditioned solve: the closest points are either an
+// endpoint of one segment and a point of the other (four point-segment distances: clamped projections, well conditioned),
+// or interior to both, and then the distance is that of the two lines, |w . (u x v)| / |u x v|. The line distance is used
+// whenever the closest points of the lines may be interior (1 mm of tolerance on their parameters). Within ~0.6 degrees
+// of parallel, where fp32 cannot resolve the lines' distance, the endpoint distance less what sliding along both segments
+// can gain bounds it instead. The fp32 error of every term is below 3e-6 m at these sizes; the 1e-5 m of slack is ten
+// times MPR's tolerance.
+LS_DEV float point_seg_dist2(const float* p, const float* u, float h) {
+  const float uu = dot3(u, u), t = fminf(fmaxf(dot3(p, u) / uu, -h), h);
+  const float q[3] = {p[0] - t * u[0], p[1] - t * u[1], p[2] - t * u[2]};
+  return dot3(q, q);
+}
+LS_DEV bool capsule_hulls_apart(const float* d, const float* m1, int t1, const float* s1, const float* m2, int t2,
+                                const float* s2, float margin) {
+  const float h1 = t1 == LS_GEOM_SPHERE ? 0.0f : s1[1], h2 = t2 == LS_GEOM_SPHERE ? 0.0f : s2[1];
+  const float u[3] = {m1[2], m1[5], m1[8]}, v[3] = {m2[2], m2[5], m2[8]};
+  // endpoints of each segment against the other (relative to the other segment's centre)
+  float p[3] = {-d[0] + h1 * u[0], -d[1] + h1 * u[1], -d[2] + h1 * u[2]};       // pos1 + h1 u - pos2
+  float dist2 = point_seg_dist2(p, v, h2);
+  for (int k = 0; k < 3; k++) p[k] = -d[k] - h1 * u[k];
+  dist2 = fminf(dist2, point_seg_dist2(p, v, h2));
+  for (int k = 0; k < 3; k++) p[k] = d[k] + h2 * v[k];                            // pos2 + h2 v - pos1
+  dist2 = fminf(dist2, point_seg_dist2(p, u, h1));
+  for (int k = 0; k < 3; k++) p[k] = d[k] - h2 * v[k];
+  dist2 = fminf(dist2, point_seg_dist2(p, u, h1));
+  if (h1 > 0 && h2 > 0) {
+    // closest points of the lines pos1 + s u, pos2 + t v; w = pos1 - pos2
+    const float a = dot3(u, u), e = dot3(v, v), b = dot3(u, v), c = -dot3(u, d), f = -dot3(v, d);
+    float n[3];
+    cross3(n, u, v);
+    const float nn = dot3(n, n);
+    if (nn < 1e-4f * a * e) {
+      // nearly parallel: from interior closest points, slide both parameters alike (t against s if the axes are
+      // antiparallel) until one reaches an endpoint: the distance grows by at most that slide times |u -+ v|
+      const float sg = b >= 0 ? 1.0f : -1.0f, w[3] = {u[0] - sg * v[0], u[1] - sg * v[1], u[2] - sg * v[2]};
+      const float lb = fmaxf(sqrtf(dist2) - 2.0f * fmaxf(h1, h2) * sqrtf(dot3(w, w)), 0.0f);
+      dist2 = lb * lb;
+    } else {
+      const float den = a * e - b * b, s = (b * f - c * e) / den, t = (a * f - b * c) / den;
+      if (fabsf(s) <= h1 + 1e-3f && fabsf(t) <= h2 + 1e-3f) {
+        const float wn = dot3(d, n);
+        dist2 = fminf(dist2, wn * wn / nn);
+      }
+    }
+  }
+  const float rr = s1[0] + s2[0] + margin + 1e-5f;
+  return dist2 > rr * rr;
+}
+
 // second filter of a general convex pair that passed the bounding spheres
 template <class C>
 LS_FN bool convex_obb_filter(const int ms, const EnvS<C>& e, int p) {
@@ -1267,6 +1326,23 @@ LS_FN bool convex_obb_filter(const int ms, const EnvS<C>& e, int p) {
     }
   }
   return true;
+}
+
+// Third filter of a box-test survivor with pair flag 4 (sphere | capsule | cylinder vs cylinder, locosim_host.h): a box
+// bounds a thin cylinder poorly next to a slanted capsule, and without this test such near misses each cost a job
+// (UnitreeA1: the front hips' cylinders against the front legs). Rejecting a pair only skips MPR, which would not have
+// reported a contact for it; its separating-direction cache entry (which, too, only ever skips MPR) is not refreshed.
+// A stage of its own, called only for flagged pairs: models without them run the box test's code as before.
+template <class C>
+LS_FN bool convex_hull_filter(const int ms, const EnvS<C>& e, int p) {
+  const DevModel& m = c_models[ms];
+  const int g1 = m.pair_geom[2 * p], g2 = m.pair_geom[2 * p + 1];
+  const float d[3] = {e.gxpos[g2][0] - e.gxpos[g1][0], e.gxpos[g2][1] - e.gxpos[g1][1], e.gxpos[g2][2] - e.gxpos[g1][2]};
+  float RA[9], RB[9];
+  geom_mat(ms, e, g1, RA);
+  geom_mat(ms, e, g2, RB);
+  return !capsule_hulls_apart(d, RA, m.geom_type[g1], m.geom_size + 3 * g1, RB, m.geom_type[g2], m.geom_size + 3 * g2,
+                              fmaxf(m.geom_margin[g1], m.geom_margin[g2]));
 }
 
 // contact parameters (mj_contactParam), frame completion (mju_makeFrame) and storage of one raw contact
@@ -1379,6 +1455,7 @@ LS_DEV int box_box_edge(float margin, const float* p1, const float* m1, const fl
 //                                2 MPR ran, no contact; res[1..3] = the last direction tested (refreshes o's cache),
 //                                3 MPR ran, touching contact without a normal (ignored).
 #define LS_MAXJOB 32
+#define LS_CAND_HULL(pk) (((pk) >> 11) & 0x8000)     // pair flag 4 (bit 26 of pair_packed) as bit 15 of a candidate entry
 template <class C>
 LS_FN void convex_job(const int ms, const EnvS<C>& o, EnvS<C>& e, int p, float* res) {
   const DevModel& m = c_models[ms];
@@ -1565,6 +1642,7 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
   // by pair among themselves); the order of constraint rows has no influence on the solution.
   // Layout of the 5 * MAXEFC floats: [results: LS_MAXJOB x 8 floats][candidate / job list: unsigned short ...].
   float* jobres = e.r_D;
+  // (C::HULL: candidate entries carry pair flag 4 in bit 15 until the box test; job entries are plain pair indices)
   unsigned short* cand = reinterpret_cast<unsigned short*>(e.r_D + 8 * LS_MAXJOB);
   const int cand_max = (int)((5 * EnvS<C>::MAXEFC - 8 * LS_MAXJOB) * sizeof(float) / sizeof(unsigned short));
   static_assert(5 * EnvS<C>::MAXEFC - 8 * LS_MAXJOB >= 128, "room for the candidate list");
@@ -1573,7 +1651,7 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
   for (int p = 0; p < m.np; p++) {
     const int pk = e.pk_tab[p];
     if (!pair_filter(ms, e, p, pk)) continue;
-    if (pk & (2 << 24)) { if (ncand < cand_max) cand[ncand++] = (unsigned short)p; continue; }
+    if (pk & (2 << 24)) { if (ncand < cand_max) cand[ncand++] = (unsigned short)(p | (C::HULL ? LS_CAND_HULL(pk) : 0)); continue; }
     RawCon raw[4];
     int g1, g2; float margin;
     const int n = pair_narrow(ms, e, p, raw, &g1, &g2, &margin);
@@ -1583,7 +1661,12 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
   }
   {
     int nsurv = 0;
-    for (int k = 0; k < ncand; k++) if (convex_obb_filter(ms, e, cand[k])) cand[nsurv++] = cand[k];
+    for (int k = 0; k < ncand; k++) {
+      const int p = cand[k] & 0x7fff;
+      if (convex_obb_filter(ms, e, p) && (!C::HULL || !(cand[k] & 0x8000) || (c_debug & 32) || convex_hull_filter(ms, e, p)))
+        cand[nsurv++] = (unsigned short)p;
+    }
+    g_obb_pass += nsurv;                       // (the jobs of this evaluation)
     float tmp[8];
     for (int base = 0; base < nsurv; base += LS_MAXJOB) {
       const int nj = nsurv - base < LS_MAXJOB ? nsurv - base : LS_MAXJOB;
@@ -1599,11 +1682,15 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
   // The pair table holds the primitive pairs first (ModelPack order: modelpack.pack partitions it), then the general convex
   // pairs: the latter only need the bounding-sphere test and a compaction, a lean loop (2 rounds of 32 per iteration).
   const int np_prim = m.np_prim;
+  PH_T0(tc);
   for (int base = 0; base < np_prim; base += 32) {
+    PH_LAP(PH_COL_PRIM_NARROW, tc);                     // (the previous round's narrow phase)
     const int p = base + lane;
     const int pk = p < np_prim ? e.pk_tab[p] : 0;
     bool hit = (p < np_prim) && pair_filter(ms, e, p, pk);
-    if (!__any_sync(0xffffffffu, hit)) continue;        // (most rounds of 32 pairs have no candidate at all)
+    const bool any = __any_sync(0xffffffffu, hit);
+    PH_LAP(PH_COL_PRIM_FILTER, tc);
+    if (!any) continue;                                 // (most rounds of 32 pairs have no candidate at all)
     RawCon raw[4];
     int g1 = 0, g2 = 0, n = 0, nact = 0;
     float margin = 0, incl = 0;
@@ -1634,6 +1721,7 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
     LANE0 { const int nc = e.ncon + total; e.ncon = nc < EnvS<C>::MAXCON ? nc : EnvS<C>::MAXCON; }
     __syncwarp();
   }
+  PH_LAP(PH_COL_PRIM_NARROW, tc);
   if (C::CONVEX && !(c_debug & 4)) {
     const int npt = m.np;
     NOUNROLL for (int base = np_prim; base < npt; base += 64) {
@@ -1652,66 +1740,80 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
       if (ma | mb) {
         const unsigned lt = (1u << lane) - 1u;
         const int sa = ncand + __popc(ma & lt), sb = ncand + __popc(ma) + __popc(mb & lt);
-        if (ha && sa < cand_max) cand[sa] = (unsigned short)pa;
-        if (hb && sb < cand_max) cand[sb] = (unsigned short)pb;
+        if (ha && sa < cand_max) cand[sa] = (unsigned short)(pa | (C::HULL ? LS_CAND_HULL(ka) : 0));
+        if (hb && sb < cand_max) cand[sb] = (unsigned short)(pb | (C::HULL ? LS_CAND_HULL(kb) : 0));
         ncand += __popc(ma) + __popc(mb);
       }
     }
   }
+  PH_LAP(PH_COL_SPHERES, tc);
   if (C::CONVEX) {
     if (ncand > cand_max) ncand = cand_max;
     __syncwarp();
     // (1) oriented-box test on the compacted candidates; the survivors are compacted in place (pair order is kept)
     int nsurv = 0;
     NOUNROLL for (int base = 0; base < ncand; base += 32) {
-      const int p = base + lane < ncand ? (int)cand[base + lane] : -1;
-      const bool pass = p >= 0 && ((c_debug & 2) || convex_obb_filter(ms, e, p));
+      const int c = base + lane < ncand ? (int)cand[base + lane] : -1, p = C::HULL ? c & 0x7fff : c;
+      bool pass = c >= 0 && ((c_debug & 2) || convex_obb_filter(ms, e, p));
+      if (C::HULL && pass && (c & 0x8000) && !(c_debug & 32)) pass = convex_hull_filter(ms, e, p);
       const unsigned pm = __ballot_sync(0xffffffffu, pass);
       __syncwarp();                              // (all 32 entries are read before the in-place compaction overwrites any)
       if (pass) cand[nsurv + __popc(pm & ((1u << lane) - 1u))] = (unsigned short)p;      // (slot <= base + lane: in place is safe)
       nsurv += __popc(pm);
       __syncwarp();
     }
+    PH_LAP(PH_COL_OBB, tc);
+    PH_CNT(PH_COL_NOBB, nsurv);
     if (c_debug & 1) nsurv = 0;
     // (2) the block's warps share the jobs: every env publishes its first LS_MAXJOB survivors, all warps drain the queue
     //     (dynamic: one shared-memory atomic per job), results land in the OWNER's record list. Block barriers: every
-    //     warp of the block runs collision() the same number of times (ghost warps included).
+    //     warp of the block runs collision() the same number of times (ghost warps included). C::HULL: the first barrier
+    //     tells every warp whether any env of the block has a job: if none has, that barrier is the only one, and nobody
+    //     reads the counts (a warp that runs ahead to its next evaluation may overwrite its count at once).
     EnvS<C>* blk = &e - (threadIdx.x >> 5);
     const int nw = (int)(blockDim.x >> 5);
     const int nj = nsurv < LS_MAXJOB ? nsurv : LS_MAXJOB;
+    PH_CNT(PH_COL_NJOBS, nj);
     LANE0 { e.njobs = nj; }
     PH_T0(t);
-    __syncthreads();
-    int incl = lane < nw ? blk[lane].njobs : 0;
-    __syncthreads();        // (everybody has read the counts: a warp that runs ahead may publish its next evaluation's count)
-    const int mine = incl;
+    bool any_jobs = true;
+    if (C::HULL) any_jobs = __syncthreads_or(nj > 0);
+    else __syncthreads();
+    PH_LAP(PH_COL_QWAIT, tc);
+    if (any_jobs) {
+      int incl = lane < nw ? blk[lane].njobs : 0;
+      __syncthreads();      // (everybody has read the counts: a warp that runs ahead may publish its next evaluation's count)
+      const int mine = incl;
 #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += t;
-    }
-    const int total = __shfl_sync(0xffffffffu, incl, 31);
-    if (total > 0) {
-      for (;;) {
-        int g = 0;
-        if (lane == 0) g = atomicAdd(&blk[0].job_head, 1);
-        g = __shfl_sync(0xffffffffu, g, 0);
-        if (g >= total) break;
-        const int owner = __popc(__ballot_sync(0xffffffffu, incl <= g));         // first lane whose inclusive prefix exceeds g
-        const int first = __shfl_sync(0xffffffffu, incl - mine, owner);
-        EnvS<C>& o = blk[owner];
-        const unsigned short* ocand = reinterpret_cast<const unsigned short*>(o.r_D + 8 * LS_MAXJOB);
-        convex_job(ms, o, e, (int)ocand[g - first], o.r_D + 8 * (g - first));
+      for (int d = 1; d < 32; d <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= d) incl += t;
       }
-      __syncthreads();
-      PH_LAP(PH_CONVEX_QUEUE, t);
-      if (threadIdx.x == 0) blk[0].job_head = 0;       // (next use is behind the next evaluation's first barrier)
-      // (3) owners consume their records in pair order
-      NOUNROLL for (int j = 0; j < nj; j++) {
-        float rec[8];
-        for (int k = 0; k < 8; k++) rec[k] = jobres[8 * j + k];
-        __syncwarp();
-        convex_consume(ms, e, (int)cand[j], rec);
+      const int total = __shfl_sync(0xffffffffu, incl, 31);
+      if (total > 0) {      // (C::HULL: always true here, but without it ptxas saves more registers around forward()'s calls)
+        for (;;) {
+          int g = 0;
+          if (lane == 0) g = atomicAdd(&blk[0].job_head, 1);
+          g = __shfl_sync(0xffffffffu, g, 0);
+          if (g >= total) break;
+          const int owner = __popc(__ballot_sync(0xffffffffu, incl <= g));         // first lane whose inclusive prefix exceeds g
+          const int first = __shfl_sync(0xffffffffu, incl - mine, owner);
+          EnvS<C>& o = blk[owner];
+          const unsigned short* ocand = reinterpret_cast<const unsigned short*>(o.r_D + 8 * LS_MAXJOB);
+          convex_job(ms, o, e, (int)ocand[g - first], o.r_D + 8 * (g - first));
+        }
+        PH_LAP(PH_COL_JOBS, tc);
+        __syncthreads();
+        PH_LAP(PH_CONVEX_QUEUE, t);
+        PH_LAP(PH_COL_JOBS_WAIT, tc);
+        if (threadIdx.x == 0) blk[0].job_head = 0;       // (next use is behind the next evaluation's first barrier)
+        // (3) owners consume their records in pair order
+        NOUNROLL for (int j = 0; j < nj; j++) {
+          float rec[8];
+          for (int k = 0; k < 8; k++) rec[k] = jobres[8 * j + k];
+          __syncwarp();
+          convex_consume(ms, e, (int)cand[j], rec);
+        }
       }
     }
     // (4) overflow (more than LS_MAXJOB survivors in one evaluation: not seen in the in-scope models): the owner alone
@@ -1723,6 +1825,7 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
       __syncwarp();
       convex_consume(ms, e, (int)cand[j], rec);
     }
+    PH_LAP(PH_COL_CONSUME, tc);
   }
 #endif
   SYNC();

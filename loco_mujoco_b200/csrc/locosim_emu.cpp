@@ -146,7 +146,15 @@ void emu_set_dof(EmuBase* s, float* out) {
   s->act.assign(s->m.nu > 0 ? s->m.nu : 1, 0.0f);
   s->dof.out = out;
 }
-long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, 0}; return v[k]; }
+long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, g_obb_pass}; return v[k]; }
+// the diagnostic switches of the emulated engine (LOCOSIM_DEBUG; e.g. 32: no capsule-hull test)
+void emu_set_debug(int v) { c_debug = v; }
+// capsule_hulls_apart of two geoms (type, position, row-major frame, geom_size) with the pair's margin
+int emu_capsule_hulls_apart(int t1, const float* pos1, const float* m1, const float* s1, int t2, const float* pos2,
+                            const float* m2, const float* s2, float margin) {
+  const float d[3] = {pos2[0] - pos1[0], pos2[1] - pos1[1], pos2[2] - pos1[2]};
+  return capsule_hulls_apart(d, m1, t1, s1, m2, t2, s2, margin) ? 1 : 0;
+}
 long emu_ls_evals() { return g_ls_evals; }
 long emu_ls_searches() { return g_ls_searches; }
 int emu_ncon(EmuBase* s) { return s->info(0); }

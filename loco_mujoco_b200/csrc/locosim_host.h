@@ -86,8 +86,10 @@ static inline std::string parse_model(HostModel& h, const int* ints, int n_ints,
   h.ints.insert(h.ints.end(), frow.begin(), frow.end());
   for (int i = 0; i < 32; i++) for (int j = 0; j <= i; j++) h.ints.push_back((i << 8) | j);   // row-major lower triangle, n <= 32
   // packed candidate-pair table of the mid-phase: g1 | g2 << 12 | flags << 24 (1: g1 is a plane, 2: general convex
-  // pair) and, as float bits, the bound of the bounding-sphere test (rbound[g2] for planes, else rbound[g1] + rbound[g2])
+  // pair, 4: capsule-hull test) and, as float bits, the bound of the bounding-sphere test (rbound[g2] for planes, else
+  // rbound[g1] + rbound[g2])
   if (ng >= 4096) return "more than 4095 geoms";
+  if (np >= 32768) return "more than 32767 candidate pairs";         // (15-bit pair index in collision()'s candidate list)
   h.np_prim = np;
   bool seen_convex = false;
   for (int p = 0; p < np; p++) {
@@ -101,6 +103,10 @@ static inline std::string parse_model(HostModel& h, const int* ints, int n_ints,
       const bool prim = (t1 == LS_GEOM_SPHERE && (t2 == LS_GEOM_SPHERE || t2 == LS_GEOM_CAPSULE || t2 == LS_GEOM_BOX)) ||
                         (t1 == LS_GEOM_CAPSULE && t2 == LS_GEOM_CAPSULE);
       if (!prim) flags |= 2;
+      // 4: a general convex pair of axial geoms (sphere | capsule | cylinder vs cylinder): its box test is followed by the
+      // exact capsule-hull test (locosim_core.cuh convex_hull_filter)
+      auto axial = [](int t) { return t == LS_GEOM_SPHERE || t == LS_GEOM_CAPSULE || t == LS_GEOM_CYLINDER; };
+      if (!prim && axial(t1) && axial(t2)) flags |= 4;
     }
     if (flags & 2) { if (!seen_convex) h.np_prim = p; seen_convex = true; }
     else if (seen_convex) return "candidate pairs not partitioned (primitive pairs first, general convex pairs last: modelpack.pack)";

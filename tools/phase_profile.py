@@ -25,8 +25,15 @@ os.environ.setdefault("LOCO_MUJOCO_B200_FORCE_BUNDLED", "1")
 PHASES = ["kinematics", "com_pos", "crb_factor", "smooth_forces", "collision", "convex_queue", "make_constraint", "warmstart",
           "newton_wait", "newton_trips", "newton_iters", "make_hessian", "chol_factor", "chol_solve", "line_search", "ls_eval",
           "ls_evals", "update_constraint", "update_gradient", "newton_tail", "integrator", "substep", "substeps", "prologue",
-          "epilogue", "groups"]
-COUNTS = {"newton_trips", "newton_iters", "ls_evals", "substeps", "groups"}
+          "epilogue", "groups",
+          # collision() split: primitive filter rounds, primitive narrow phase + fill_contact, convex bounding spheres, box
+          # (and capsule-hull) tests, the job queue's first barrier, own jobs, the wait for the block's other jobs,
+          # convex_consume; counts of box-test survivors and of jobs published
+          "col_prim_filter", "col_prim_narrow", "col_spheres", "col_obb", "col_queue_wait", "col_jobs", "col_jobs_wait",
+          "col_consume", "col_obb_survivors", "col_jobs_published"]
+COUNTS = {"newton_trips", "newton_iters", "ls_evals", "substeps", "groups", "col_obb_survivors", "col_jobs_published"}
+COLLISION_SPLIT = ["col_prim_filter", "col_prim_narrow", "col_spheres", "col_obb", "col_queue_wait", "col_jobs",
+                   "col_jobs_wait", "col_consume"]
 
 
 def build_diagnostic(tmp):
@@ -62,6 +69,10 @@ def table(raw):
         "lockstep_trips_per_solve": c["newton_trips"] / n,
         "lockstep_efficiency": c["newton_iters"] / max(1, c["newton_trips"]),
         "ls_evals_per_iteration": c["ls_evals"] / iters,
+        "collision_split_cycles": {k: cyc[k] for k in COLLISION_SPLIT},
+        "collision_unsplit_cycles": cyc["collision"] - sum(cyc[k] for k in COLLISION_SPLIT),
+        "convex_jobs_per_env_substep": c["col_jobs_published"] / n,
+        "box_test_survivors_per_env_substep": c["col_obb_survivors"] / n,
         "env_substeps": c["substeps"], "groups": c["groups"],
         "prologue_epilogue_cycles_per_group": (c["prologue"] + c["epilogue"]) / max(1, c["groups"]),
     }
