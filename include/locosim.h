@@ -218,6 +218,40 @@ int locosim_set_dof_outputs(locosim_t* h, float* d_dof);
 int locosim_dataset_rows(const locosim_t* h);
 int locosim_create_dataset(locosim_t* h, float* d_states, float* d_next_states, float* d_last, void* stream);
 
+/* Reference outputs: the body outputs of the mocap clip, the expert side of body-space imitation terms (end-effector and
+ * centre-of-mass tracking, keypoint discriminators, foot placement). Caller-owned DEVICE buffers, each fp32
+ * [n_envs, nbody, LS_BODY_DIM]; a REFERENCE ROW has the layout and body indices of the body outputs above.
+ * The reference row of an env is the body outputs of the state locosim_reset_rows would give it if it were reset onto the
+ * table row (traj, sample) at its cursor (locosim_get_cursor): reset_value of that row, i.e. root x / y zeroed and, under
+ * setup_random_rot, the yaw shifted and root (vx, vy) rotated by the rotation angle of the env's CURRENT episode (the one its
+ * last reset drew or was given by locosim_set_reset_rotation), evaluated with the env's current parameter-pool row.
+ * So immediately after any reset the reference row equals d_next_body of the same env bit for bit. Positions are therefore
+ * root-x/y-relative: to compare a simulated body with its reference, subtract the simulated root's x / y first, e.g.
+ *   foot = body[i, b, 0:3];  foot.x -= body[i, root, 0];  foot.y -= body[i, root, 1];
+ *   err  = |foot - ref[i, b, 0:3]|      (the reference root stands at x = y = 0)
+ * Phase = the cursor: it advances by one sample per control step under LS_REWARD_TRACKING or end_of_trajectory
+ * (locosim_set_time_limit), clamped at the last sample. With neither, the cursor stays on the reset row and so does the
+ * reference (this is not refused here).
+ *   d_ref:      written by every locosim_step for the state d_obs describes: for an env that ended, the cursor its terminal
+ *               step reached, before the auto-reset moves the cursor (and that episode's angle and pool row); for a
+ *               non-finite env all zeros, as in d_body.
+ *   d_next_ref: the state to act on next: written by locosim_step after the auto-reset (rows of envs not reset equal d_ref bit
+ *               for bit) and by locosim_reset* for the masked envs. locosim_set_state moves no cursor and does not write it.
+ * Either may be NULL; NULL, NULL = off = the state after locosim_create: nothing is written or launched, and no other output
+ * changes by a bit; with buffers registered no other output, the body outputs included, changes by a bit either. The rows are
+ * written by the body outputs' kernel after the step, so the launch and CUDA-graph rules are those of the body outputs:
+ * register outside of stream capture, and capture the step again after turning the feature on (a graph captured while
+ * neither body nor reference outputs were registered writes neither, and its replays do not keep the per-env record the
+ * terminal rows are built from; registering again rebuilds that record). Registering reads every env's current state on the
+ * device and waits for it; a new parameter pool (locosim_set_param_pool) does the same. */
+int locosim_set_reference_outputs(locosim_t* h, float* d_ref, float* d_next_ref);
+
+/* The reference rows of the whole dataset, row-aligned with locosim_create_dataset: d_body / d_next_body fp32
+ * [locosim_dataset_rows, nbody, LS_BODY_DIM]. Row r is the reference row of dataset row r's (traj, sample) in d_body and of
+ * (traj, sample + 1) in d_next_body, with rotation angle 0 and the compiled model's own parameters (what an env runs with when
+ * no parameter pool is set). Stream-ordered; the expert side of a body-space discriminator. */
+int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_body, void* stream);
+
 /* Per-episode goal features (UnitreeA1: cos / sin of the goal direction and the goal speed, GoalDirectionVelocity set in
  * setup() unitreeA1.py:287-291); normally loaded from the reset table, settable for reset(obs=...) (base.py:217-218,633-654).
  * d_goal fp32 [n_envs, 4]. */

@@ -36,6 +36,18 @@ struct EngineState {
   int pool_K;
 };
 
+// reference outputs of a handle (locosim_set_reference_outputs): caller-owned [N, nb, LS_BODY_DIM] reference rows of the
+// returned state (`ref`) and of the state to act on next (`next_ref`), NULL = not written; key [N] (engine-owned, NULL = the
+// feature is off): what body_kernel last wrote the env's reference rows from, i.e. what the state to act on next is
+// compared with: x = cursor, y = rotation angle (fp32 bits), z = parameter-pool row, w = the env's non-finite count
+// (counters[4]). The step kernels never read it (a table of its own, like c_bodyout).
+struct DevRefOut {
+  float* ref;
+  float* next_ref;
+  int4* key;
+};
+__constant__ DevRefOut c_refout[LS_MAX_SLOTS];
+
 __device__ __forceinline__ uint64_t mix64(uint64_t z) {
   z += 0x9E3779B97F4A7C15ULL;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
@@ -56,6 +68,15 @@ __device__ __forceinline__ float draw_rot_angle(uint64_t seed, int64_t genv, int
   return (float)(r >> 40) * (6.283185307179586f / 16777216.0f);
 }
 
+// rotation angle of the episode that reset number `episode` - 1 started (st.episode = `episode` while it runs): the one
+// reset_kernel pinned (rot_pin: episode number, angle bits; locosim_set_reset_rotation), or the counter-based draw
+__device__ __forceinline__ float episode_angle(const DevTask& t, const int2* rot_pin, uint64_t seed, int64_t genv, int env,
+                                               int episode) {
+  if (t.rot[0] < 0 || episode <= 0) return 0.0f;
+  const int2 pin = rot_pin[env];
+  return pin.x == episode ? __int_as_float(pin.y) : draw_rot_angle(seed, genv, episode - 1);
+}
+
 __device__ __forceinline__ int draw_pool_row(uint64_t seed, int64_t genv, int episode, int K) {
   if (K <= 1) return 0;
   uint64_t r = mix64((seed + 0x5DEECE66DULL) ^ mix64((uint64_t)genv * 0x100000001B3ULL + (uint64_t)(uint32_t)episode));
@@ -68,7 +89,7 @@ __device__ __forceinline__ int draw_pool_row(uint64_t seed, int64_t genv, int ep
 // ----------------------------------------------------------------------------------------------------------
 __global__ void reset_kernel(int ms, DevTask t, EngineState st, const uint8_t* mask, const int* traj_no,
                              const int* step_no, const int* pool_row, float* obs, int n_envs, uint64_t seed,
-                             int64_t env_off) {
+                             int64_t env_off, int2* rot_pin) {
   int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (env >= n_envs) return;
@@ -108,6 +129,7 @@ __global__ void reset_kernel(int ms, DevTask t, EngineState st, const uint8_t* m
     st.dr_row[env] = prow;
     st.cursor[env] = tr * t.traj_len + sp;
     *reinterpret_cast<int2*>(&st.ep[env]) = make_int2(0, 0);
+    if (st.rot_angle && t.rot[0] >= 0) rot_pin[env] = make_int2(ep + 1, __float_as_int(angle));   // (episode_angle)
   }
 }
 #endif
@@ -833,9 +855,10 @@ __global__ void __launch_bounds__(512, 1) persist_kernel(int ms, DevTask t, Solv
 }
 
 // ----------------------------------------------------------------------------------------------------------
-// Body-output kernel (locosim_set_body_outputs), one warp and one EnvS per block, from the engine's state (the env's
-// parameter-pool row as in the step kernels: masses and inertial frames differ per env under domain randomisation and carry
-// tasks). After a step (done = that step's done bytes, every env): d_next_body, and d_body of the envs the step did not
+// Body-output kernel (locosim_set_body_outputs, locosim_set_reference_outputs), one warp and one EnvS per block, from the
+// engine's state (the env's parameter-pool row as in the step kernels: masses and inertial frames differ per env under
+// domain randomisation and carry tasks). `parts`: 1 = body rows, 2 = reference keys, 4 = reference rows (with 2).
+// Body rows. After a step (done = that step's done bytes, every env): d_next_body, and d_body of the envs the step did not
 // reset (the same state). The envs the step reset are those with a done byte under auto_reset, and those reset_env marked
 // (a non-finite env) without it; reset_env has written their d_body rows from the terminal state, which the stored state no
 // longer holds. After locosim_reset* (the envs of `mask`) and locosim_set_state (all, done = NULL): d_next_body.
@@ -843,37 +866,89 @@ __global__ void __launch_bounds__(512, 1) persist_kernel(int ms, DevTask t, Solv
 // and reset_env is a call those kernels already make; a body-output call of their own, in every epilogue, changes their
 // register allocation and stack frames, which the off path must not pay for. This kernel is enqueued only while buffers
 // are registered.
+// Reference rows: the body outputs of the reset state of the table row at the env's cursor (reference_outputs), with the
+// rotation angle of its episode and its parameter-pool row. The step kernels keep nothing for them: the terminal rows of an
+// env the step reset come from the key this kernel stored after the env's previous step or reset (DevRefOut::key), with
+// the cursor moved as the step moved it; whether the step found the env non-finite, from its non-finite count.
 // ----------------------------------------------------------------------------------------------------------
 template <class C>
-__global__ void __launch_bounds__(32) body_kernel(int ms, EngineState st, const uint8_t* __restrict__ mask,
-                                                  const uint8_t* __restrict__ done, int auto_reset) {
+__global__ void __launch_bounds__(32) body_kernel(int ms, DevTask t, EngineState st, const uint8_t* __restrict__ mask,
+                                                  const uint8_t* __restrict__ done, int auto_reset, int parts, uint64_t seed,
+                                                  int64_t env_off, const int2* __restrict__ rot_pin) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int env = blockIdx.x, lane = threadIdx.x & 31;
   if (mask && !mask[env]) return;
   EnvS<C>& e = *reinterpret_cast<EnvS<C>*>(smem_raw);
   const DevModel& m = c_models[ms];
-  const DevBodyOut bo = c_bodyout[ms];
   const int nv = m.nv;
   const size_t off = (size_t)env * m.nb * LS_BODY_DIM;
-  float* body = nullptr;
-  if (done && bo.body) {
-    // (under auto_reset the done byte alone decides: a mark left by a step that was not followed by this kernel cannot
-    // hide a row; every mark is cleared here)
-    const int mark = bo.reset_mark[env];
-    const bool was_reset = done[env] != 0 && (auto_reset || mark != 0);
+  if (parts & 1) {
+    const DevBodyOut bo = c_bodyout[ms];
+    float* body = nullptr;
+    if (done && bo.body) {
+      // (under auto_reset the done byte alone decides: a mark left by a step that was not followed by this kernel cannot
+      // hide a row; every mark is cleared here)
+      const int mark = bo.reset_mark[env];
+      const bool was_reset = done[env] != 0 && (auto_reset || mark != 0);
+      __syncwarp();
+      if (!was_reset) body = bo.body + off;
+      if (lane == 0 && mark) bo.reset_mark[env] = 0;
+    }
+    float* next = bo.next_body ? bo.next_body + off : nullptr;
+    if (body || next) {
+      if (lane == 0) e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
+      for (int i = lane; i < nv; i += 32) {
+        e.qpos[i] = st.qpos[(size_t)env * nv + i];
+        e.qvel[i] = st.qvel[(size_t)env * nv + i];
+      }
+      __syncwarp();
+      body_outputs(ms, e, body, next);
+    }
+  }
+  const DevRefOut ro = c_refout[ms];
+  if (!(parts & 2) || !ro.key) return;
+  const int ncol = 2 * nv + t.n_goal;
+  const int4 key = ro.key[env];
+  const int cur = st.cursor[env], prow = st.dr_row[env], nbad = st.counters[(size_t)env * 8 + 4];
+  const float angle = episode_angle(t, rot_pin, seed, env_off + env, env, st.episode[env]);
+  float* ref = (parts & 4) && done && ro.ref ? ro.ref + off : nullptr;
+  float* next = (parts & 4) && ro.next_ref ? ro.next_ref + off : nullptr;
+  if (ref && done[env] != 0 && (auto_reset || nbad != key.w)) {
+    // the step reset the env: d_ref describes the state it ended in, i.e. the key it started from with the cursor moved
+    // once (clamped) under LS_REWARD_TRACKING or end_of_trajectory, as step_epilogue moves it; zeros where it found the
+    // env non-finite
+    if (nbad != key.w) {
+      for (int k = lane; k < m.nb * LS_BODY_DIM; k += 32) ref[k] = 0.0f;
+    } else {
+      int c = key.x;
+      if ((t.reward_type == LS_REWARD_TRACKING || st.end_of_trajectory) && c % t.traj_len + 1 < t.traj_len) c += 1;
+      if (lane == 0) e.prm = st.pool + (size_t)key.z * m.pool_P;
+      reference_outputs(ms, t, e, t.table + (size_t)c * ncol, __int_as_float(key.y), ref, (float*)nullptr);
+    }
+    ref = nullptr;
+  }
+  if (ref || next) {
     __syncwarp();
-    if (!was_reset) body = bo.body + off;
-    if (lane == 0 && mark) bo.reset_mark[env] = 0;
+    if (lane == 0) e.prm = st.pool + (size_t)prow * m.pool_P;
+    reference_outputs(ms, t, e, t.table + (size_t)cur * ncol, angle, ref, next);
   }
-  float* next = bo.next_body ? bo.next_body + off : nullptr;
-  if (!body && !next) return;
-  if (lane == 0) e.prm = st.pool + (size_t)st.dr_row[env] * m.pool_P;
-  for (int i = lane; i < nv; i += 32) {
-    e.qpos[i] = st.qpos[(size_t)env * nv + i];
-    e.qvel[i] = st.qvel[(size_t)env * nv + i];
-  }
-  __syncwarp();
-  body_outputs(ms, e, body, next);
+  if (lane == 0) ro.key[env] = make_int4(cur, __float_as_int(angle), prow, nbad);
+}
+
+// Reference rows of the dataset (locosim_create_dataset_bodies), one warp and one EnvS per block and dataset row: row r of
+// locosim_create_dataset is (traj, sample) -> (traj, sample + 1); angle 0, parameters `prm` (the compiled model's own).
+template <class C>
+__global__ void __launch_bounds__(32) dataset_body_kernel(int ms, DevTask t, const float* __restrict__ prm,
+                                                          float* __restrict__ body, float* __restrict__ next_body) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  EnvS<C>& e = *reinterpret_cast<EnvS<C>*>(smem_raw);
+  const DevModel& m = c_models[ms];
+  const int r = blockIdx.x, per = t.traj_len - 1, tj = r / per, sp = r - tj * per, ncol = 2 * m.nv + t.n_goal;
+  const float* row = t.table + ((size_t)tj * t.traj_len + sp) * ncol;
+  const size_t off = (size_t)r * m.nb * LS_BODY_DIM;
+  if ((threadIdx.x & 31) == 0) e.prm = prm;
+  reference_outputs(ms, t, e, row, 0.0f, body + off, (float*)nullptr);
+  reference_outputs(ms, t, e, row + ncol, 0.0f, next_body + off, (float*)nullptr);
 }
 
 // ----------------------------------------------------------------------------------------------------------
@@ -923,6 +998,10 @@ struct locosim_handle {
   DevModel dm;
   DevApplied applied = {nullptr, nullptr};
   DevBodyOut bodyout = {nullptr, nullptr, nullptr};
+  DevRefOut refout = {nullptr, nullptr, nullptr};
+  int4* ref_key = nullptr;           // the reference keys [n_envs] (DevRefOut::key) once reference outputs were registered
+  int2* rot_pin = nullptr;           // [n_envs] episode number and angle of the last rotation reset_kernel was given (episode_angle)
+  float* d_model_row = nullptr;      // the compiled model's own parameter row (locosim_create_dataset_bodies), on first use
   DevContact contact = {nullptr, 1};
   DevDof dof = {nullptr, 1};
   float* dof_act = nullptr;          // the dof outputs' actuator-force scratch [n_envs, nu] (c_dof_act)
@@ -959,9 +1038,18 @@ static_assert(sizeof(EnvS<CfgPyrRK4>) * 14 <= 232448, "HumanoidTorque / Atlas: 1
 static_assert(sizeof(EnvS<CfgPyrEuler29>) * 9 <= 232448, "UnitreeG1: 9 envs per SM");
 
 template <class C>
-static int launch_body(locosim_handle* h, const uint8_t* mask, const uint8_t* done, int auto_reset, cudaStream_t s) {
+static int launch_body(locosim_handle* h, const uint8_t* mask, const uint8_t* done, int auto_reset, int parts, cudaStream_t s) {
   static_assert(sizeof(EnvS<C>) <= 48 * 1024, "body_kernel: one EnvS per block within the default shared-memory limit");
-  body_kernel<C><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, mask, done, auto_reset);
+  body_kernel<C><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->dt, h->st, mask, done, auto_reset, parts, h->seed,
+                                                        h->env_off, h->rot_pin);
+  CK(cudaGetLastError());
+  return 0;
+}
+template <class C>
+static int launch_dataset_bodies(locosim_handle* h, float* body, float* next_body, cudaStream_t s) {
+  const int rows = h->ht.n_traj * (h->ht.traj_len - 1);
+  if (rows > 0)
+    dataset_body_kernel<C><<<rows, 32, sizeof(EnvS<C>), s>>>(h->slot, h->dt, h->d_model_row, body, next_body);
   CK(cudaGetLastError());
   return 0;
 }
@@ -987,8 +1075,8 @@ static int launch_step(locosim_handle* h, const float* a, float* o, float* r, ui
                                                          h->split);
   }
   CK(cudaGetLastError());
-  // body outputs (only while registered): the rows the step kernel did not write
-  if (h->bodyout.body || h->bodyout.next_body) return launch_body<C>(h, nullptr, d, auto_reset, s);
+  // body and reference outputs (only while registered): the rows the step kernel did not write
+  if (h->bodyout.body || h->bodyout.next_body || h->refout.key) return launch_body<C>(h, nullptr, d, auto_reset, 7, s);
   return 0;
 }
 template <class C>
@@ -1151,18 +1239,24 @@ extern "C" int locosim_configs31_setup(locosim_handle* h) __attribute__((weak));
 extern "C" int locosim_configs31_step(locosim_handle* h, const float* a, float* o, float* r, uint8_t* d, float* no,
                                       int auto_reset, cudaStream_t s) __attribute__((weak));
 extern "C" int locosim_configs31_sync_model(locosim_handle* h) __attribute__((weak));
-extern "C" int locosim_configs31_body(locosim_handle* h, const uint8_t* mask, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_configs31_body(locosim_handle* h, const uint8_t* mask, int parts, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_configs31_dataset_bodies(locosim_handle* h, float* body, float* next_body, cudaStream_t s)
+    __attribute__((weak));
 
-// d_next_body rows of the envs of `mask` (NULL = all), when registered: after locosim_reset* and locosim_set_state
-static int next_body_rows(locosim_handle* h, const uint8_t* mask, cudaStream_t s) {
-  if (!h->bodyout.next_body) return 0;
+// body_kernel outside a step, for the envs of `mask` (NULL = all), the parts (see body_kernel) that are registered:
+// d_next_body (1) after locosim_reset* and locosim_set_state; the reference keys (2) and d_next_ref (4) after locosim_reset*,
+// the keys alone after a registration and a new parameter pool
+static int next_body_rows(locosim_handle* h, const uint8_t* mask, int parts, cudaStream_t s) {
+  if (!h->bodyout.next_body) parts &= ~1;
+  if (!h->refout.key) parts &= ~6;
+  if (!parts) return 0;
   switch (h->cfg) {
-    case 0: return launch_body<CfgEllEuler>(h, mask, nullptr, 0, s);
-    case 1: return launch_body<CfgPyrEuler>(h, mask, nullptr, 0, s);
-    case 3: return launch_body<CfgPyrEuler29>(h, mask, nullptr, 0, s);
+    case 0: return launch_body<CfgEllEuler>(h, mask, nullptr, 0, parts, s);
+    case 1: return launch_body<CfgPyrEuler>(h, mask, nullptr, 0, parts, s);
+    case 3: return launch_body<CfgPyrEuler29>(h, mask, nullptr, 0, parts, s);
     case 4:
-    case 5: return locosim_configs31_body(h, mask, s);
-    default: return launch_body<CfgPyrRK4>(h, mask, nullptr, 0, s);
+    case 5: return locosim_configs31_body(h, mask, parts, s);
+    default: return launch_body<CfgPyrRK4>(h, mask, nullptr, 0, parts, s);
   }
 }
 
@@ -1210,13 +1304,13 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
        cudaMalloc((void**)&h->st.episode, N * 4) == cudaSuccess && cudaMalloc((void**)&h->st.counters, N * 32) == cudaSuccess &&
        cudaMalloc((void**)&h->st.dr_row, N * 4) == cudaSuccess && cudaMalloc((void**)&h->st.perm, N * 4) == cudaSuccess &&
        cudaMalloc((void**)&h->st.cursor, N * 4) == cudaSuccess &&
-       cudaMalloc((void**)&h->st.ep, N * 16) == cudaSuccess &&
+       cudaMalloc((void**)&h->st.ep, N * 16) == cudaSuccess && cudaMalloc((void**)&h->rot_pin, N * 8) == cudaSuccess &&
        up((void**)&h->d_pool, h->hm.default_row.data(), h->hm.default_row.size() * 4);
   if (!ok) { std::string m = std::string("device allocation failed: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); g_create_error = m; return 1; }
   cudaMemset(h->st.qpos, 0, N * nv * 4); cudaMemset(h->st.qvel, 0, N * nv * 4); cudaMemset(h->st.ws, 0, N * nv * 4);
   cudaMemset(h->st.goal, 0, N * 16); cudaMemset(h->st.episode, 0, N * 4); cudaMemset(h->st.counters, 0, N * 32);
   cudaMemset(h->st.dr_row, 0, N * 4); cudaMemset(h->st.cursor, 0, N * 4);
-  cudaMemset(h->st.ep, 0, N * 16);
+  cudaMemset(h->st.ep, 0, N * 16); cudaMemset(h->rot_pin, 0, N * 8);
   h->st.max_episode_steps = 0; h->st.end_of_trajectory = 0;
   h->st.rot_angle = nullptr;
   { std::vector<int> id(N); for (size_t i = 0; i < N; i++) id[i] = (int)i; cudaMemcpy(h->st.perm, id.data(), N * 4, cudaMemcpyHostToDevice); }
@@ -1227,6 +1321,7 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
   if (cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_refout, &h->refout, sizeof(DevRefOut), sizeof(DevRefOut) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_dof_act, &h->dof_act, sizeof(float*), sizeof(float*) * h->slot) != cudaSuccess) {
@@ -1266,6 +1361,7 @@ void locosim_destroy(locosim_t* h) {
   cudaFree(h->split.carry); cudaFree(h->split.bcount); cudaFree(h->split.benv); cudaFree(h->split.seq);
   cudaFree(h->pq.carry); cudaFree(h->pq.cnt); cudaFree(h->pq.tot); cudaFree(h->pq.benv); cudaFree(h->pq.seq);
   cudaFree(h->bodyout.reset_mark);
+  cudaFree(h->ref_key); cudaFree(h->rot_pin); cudaFree(h->d_model_row);
   cudaFree(h->dof_act);
   delete h;
 }
@@ -1286,10 +1382,10 @@ int locosim_reset_rows(locosim_t* h, const uint8_t* d_mask, const int32_t* d_tra
   CK(cudaSetDevice(h->device));
   int threads = 128, blocks = (h->n_envs * 32 + threads - 1) / threads;
   reset_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(h->slot, h->dt, h->st, d_mask, d_traj, d_step, d_pool_row, d_obs,
-                                                             h->n_envs, h->seed, h->env_off);
+                                                             h->n_envs, h->seed, h->env_off, h->rot_pin);
   h->st.rot_angle = nullptr;        // pinned rotation angles apply to one reset call
   CK(cudaGetLastError());
-  return next_body_rows(h, d_mask, (cudaStream_t)stream);
+  return next_body_rows(h, d_mask, 7, (cudaStream_t)stream);
 }
 int locosim_set_reset_rotation(locosim_t* h, const float* d_angle) { h->st.rot_angle = d_angle; return 0; }
 int locosim_get_cursor(locosim_t* h, int32_t* d_out, void* stream) {
@@ -1321,6 +1417,38 @@ int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body) {
   CK(cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot));
   if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   return 0;
+}
+int locosim_set_reference_outputs(locosim_t* h, float* d_ref, float* d_next_ref) {
+  CK(cudaSetDevice(h->device));
+  const bool on = d_ref || d_next_ref;
+  if (on && !h->ref_key) CK(cudaMalloc((void**)&h->ref_key, (size_t)h->n_envs * sizeof(int4)));
+  h->refout.ref = d_ref; h->refout.next_ref = d_next_ref; h->refout.key = on ? h->ref_key : nullptr;
+  // (a __constant__ table of its own in both translation units, read by body_kernel when it runs)
+  CK(cudaMemcpyToSymbol(c_refout, &h->refout, sizeof(DevRefOut), sizeof(DevRefOut) * h->slot));
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (!on) return 0;
+  // every env's key from its current state (steps and resets keep them from here on); nothing else is written
+  CK(cudaDeviceSynchronize());
+  if (next_body_rows(h, nullptr, 2, 0)) return 1;
+  CK(cudaDeviceSynchronize());
+  return 0;
+}
+int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_body, void* stream) {
+  if (!d_body || !d_next_body) { h->err = "null buffer"; return 1; }
+  CK(cudaSetDevice(h->device));
+  if (!h->d_model_row) {
+    CK(cudaMalloc((void**)&h->d_model_row, h->hm.default_row.size() * 4));
+    CK(cudaMemcpy(h->d_model_row, h->hm.default_row.data(), h->hm.default_row.size() * 4, cudaMemcpyHostToDevice));
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (h->cfg) {
+    case 0: return launch_dataset_bodies<CfgEllEuler>(h, d_body, d_next_body, s);
+    case 1: return launch_dataset_bodies<CfgPyrEuler>(h, d_body, d_next_body, s);
+    case 3: return launch_dataset_bodies<CfgPyrEuler29>(h, d_body, d_next_body, s);
+    case 4:
+    case 5: return locosim_configs31_dataset_bodies(h, d_body, d_next_body, s);
+    default: return launch_dataset_bodies<CfgPyrRK4>(h, d_body, d_next_body, s);
+  }
 }
 int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {
   CK(cudaSetDevice(h->device));
@@ -1419,7 +1547,7 @@ int locosim_set_state(locosim_t* h, const float* q, const float* v, const float*
   if (v) CK(cudaMemcpyAsync(h->st.qvel, v, bytes, cudaMemcpyDeviceToDevice, s));
   if (w) CK(cudaMemcpyAsync(h->st.ws, w, bytes, cudaMemcpyDeviceToDevice, s));
   else CK(cudaMemsetAsync(h->st.ws, 0, bytes, s));
-  return next_body_rows(h, nullptr, s);
+  return next_body_rows(h, nullptr, 1, s);
 }
 int locosim_set_goal(locosim_t* h, const float* g, void* stream) {
   if (!g) { h->err = "null buffer"; return 1; }
@@ -1469,12 +1597,18 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
   CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
   if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   CK(cudaMemset(h->st.dr_row, 0, (size_t)h->n_envs * 4));
+  if (h->refout.key) {
+    // (the reference keys name the envs' pool rows: every env is on row 0 of the new pool now)
+    if (next_body_rows(h, nullptr, 2, 0)) return 1;
+    CK(cudaDeviceSynchronize());
+  }
   return 0;
 }
 
 int locosim_kernels_per_step(const locosim_t* h) {
   const int nsub = h->dt.n_substeps;
-  const int body = h->bodyout.body || h->bodyout.next_body ? 1 : 0;    // (body_kernel, while body outputs are registered)
+  // (body_kernel, while body or reference outputs are registered)
+  const int body = h->bodyout.body || h->bodyout.next_body || h->refout.key ? 1 : 0;
   if (h->persist) return 1 + body;
   if (h->resort < nsub) return (nsub + h->resort - 1) / h->resort + body;
   return (h->regroup ? 2 : 1) + body;

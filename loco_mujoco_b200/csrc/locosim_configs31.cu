@@ -41,6 +41,7 @@ int locosim_configs31_sync_model(Handle31* h) {
   CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
   CK(cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot));
   CK(cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot));
+  CK(cudaMemcpyToSymbol(c_refout, &h->refout, sizeof(DevRefOut), sizeof(DevRefOut) * h->slot));
   CK(cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot));
   CK(cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot));
   CK(cudaMemcpyToSymbol(c_dof_act, &h->dof_act, sizeof(float*), sizeof(float*) * h->slot));
@@ -67,11 +68,20 @@ int locosim_configs31_step(Handle31* h, const float* a, float* o, float* r, uint
   }
 }
 
-int locosim_configs31_body(Handle31* h, const uint8_t* mask, cudaStream_t s) {
+int locosim_configs31_body(Handle31* h, const uint8_t* mask, int parts, cudaStream_t s) {
   using namespace locosim31;
   switch (h->cfg) {
-    case 4: return launch_body<CfgPyrRK4_31>(h, mask, nullptr, 0, s);
-    case 5: return launch_body<CfgPyrEuler31>(h, mask, nullptr, 0, s);
+    case 4: return launch_body<CfgPyrRK4_31>(h, mask, nullptr, 0, parts, s);
+    case 5: return launch_body<CfgPyrEuler31>(h, mask, nullptr, 0, parts, s);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
+int locosim_configs31_dataset_bodies(Handle31* h, float* body, float* next_body, cudaStream_t s) {
+  using namespace locosim31;
+  switch (h->cfg) {
+    case 4: return launch_dataset_bodies<CfgPyrRK4_31>(h, body, next_body, s);
+    case 5: return launch_dataset_bodies<CfgPyrEuler31>(h, body, next_body, s);
     default: h->err = "not a 31-dof configuration"; return 1;
   }
 }

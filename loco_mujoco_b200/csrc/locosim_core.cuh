@@ -3129,6 +3129,22 @@ LS_DEV void body_rows_terminal(const int ms, EnvS<C>& e, const int env) {
   LANE0 bo.reset_mark[env] = 1;
 }
 
+// reference rows (locosim_set_reference_outputs): the body outputs of the state that a reset onto table row `row` under
+// rotation `angle` gives (reset_value: root x / y zeroed, setup_random_rot's yaw and root (vx, vy) turned), with the
+// parameters e.prm. A whole-warp call; it overwrites e.qpos / e.qvel and what body_outputs rewrites. LS_BODY_DIM floats per
+// body go to dst and to dst2 (either may be NULL).
+template <class C>
+LS_DEV void reference_outputs(const int ms, const DevTask& t, EnvS<C>& e, const float* row, float angle, float* dst,
+                              float* dst2) {
+  const int nv = c_models[ms].nv;
+  PAR_FOR(i, nv) {
+    e.qpos[i] = reset_value(t, row, nv, LS_OBS_QPOS, i, angle);
+    e.qvel[i] = reset_value(t, row, nv, LS_OBS_QVEL, i, angle);
+  }
+  SYNC();
+  body_outputs(ms, e, dst, dst2);
+}
+
 template <class C>
 LS_FN void reset_env(const int ms, const DevTask& t, EnvS<C>& e, int traj_no, int step_no, float angle) {
   const DevModel& m = c_models[ms];

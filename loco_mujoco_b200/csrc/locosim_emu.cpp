@@ -30,6 +30,7 @@ struct EmuBase {
   virtual void frames(double* gx, double* bx) = 0;
   virtual void poison() = 0;
   virtual void body(float* out) = 0;
+  virtual void ref(const DevTask& t, const float* row, float angle, float* out) = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -91,6 +92,10 @@ struct EmuT : EmuBase {
     delete keep;
   }
   void body(float* out) override { c_models[0] = m; body_outputs(0, e, out, (float*)nullptr); }
+  void ref(const DevTask& t, const float* row, float angle, float* out) override {
+    c_models[0] = m;
+    reference_outputs(0, t, e, row, angle, out, (float*)nullptr);
+  }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
 
@@ -137,6 +142,17 @@ void emu_set_ws(EmuBase* s, const double* w) { s->set_ws(w); }
 void emu_set_applied(EmuBase* s, float* xfrc, float* qfrc) { s->ap.xfrc = xfrc; s->ap.qfrc = qfrc; }
 // body outputs of the emulated env's current state (locosim_set_body_outputs): fp32 [nb, LS_BODY_DIM] into `out`
 void emu_body_outputs(EmuBase* s, float* out) { s->body(out); }
+// reference row (locosim_set_reference_outputs) of one reset-table row `row` (fp32, qpos then qvel) under rotation `angle`,
+// with the model's own parameters: fp32 [nb, LS_BODY_DIM] into `out`. recenter: the qpos indices of root x / y; rot: the
+// qpos index of the yaw and the dof indices of root vx / vy under setup_random_rot, or NULL. Leaves the emulated env in that
+// reset state.
+void emu_reference_row(EmuBase* s, const float* row, const int* recenter, const int* rot, float angle, float* out) {
+  DevTask t;
+  memset(&t, 0, sizeof(t));
+  t.recenter0 = recenter[0]; t.recenter1 = recenter[1];
+  for (int k = 0; k < 3; k++) t.rot[k] = rot ? rot[k] : -1;
+  s->ref(t, row, angle, out);
+}
 // contact outputs of the emulated env (locosim_set_contact_outputs; row 0 of the engine's layout: fp32 [nb, LS_CONTACT_DIM], or
 // NULL): every later emu_step(ctrl, nsub) runs as one control step of nsub sub-steps and leaves their mean wrench there
 void emu_set_contact(EmuBase* s, float* wrench) { s->cw.wrench = wrench; }

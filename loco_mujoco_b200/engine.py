@@ -88,6 +88,10 @@ def load_library():
     lib.locosim_set_contact_outputs.argtypes = [vp, vp]
     lib.locosim_set_dof_outputs.restype = ip
     lib.locosim_set_dof_outputs.argtypes = [vp, vp]
+    lib.locosim_set_reference_outputs.restype = ip
+    lib.locosim_set_reference_outputs.argtypes = [vp, vp, vp]
+    lib.locosim_create_dataset_bodies.restype = ip
+    lib.locosim_create_dataset_bodies.argtypes = [vp, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -100,7 +104,8 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_set_reset_rotation", "locosim_get_cursor", "locosim_dataset_rows", "locosim_create_dataset",
                     "locosim_debug_counters", "locosim_set_timeline", "locosim_set_time_limit",
                     "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
-                    "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs"]
+                    "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs",
+                    "locosim_set_reference_outputs", "locosim_create_dataset_bodies"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -182,6 +187,7 @@ class CudaEngine:
         self._body_out = (None, None)     # the registered body-output tensors (likewise)
         self._contact_out = None          # the registered contact-output tensor (likewise)
         self._dof_out = None              # the registered dof-output tensor (likewise)
+        self._ref_out = (None, None)      # the registered reference-output tensors (likewise)
         # obs / reward / done of a step live in ONE device allocation (three views), so that a consumer on the host can
         # fetch the whole step result with a single D2H copy of `packed_out`
         N, D = int(n_envs), self.obs_dim
@@ -225,7 +231,7 @@ class CudaEngine:
             self._check(self.lib.locosim_set_reset_rotation(self.h, _ptr(rot_angle)))
         self._check(self.lib.locosim_reset_rows(self.h, _ptr(mask), _ptr(traj_no), _ptr(step_no), _ptr(pool_row), _ptr(out),
                                                 self._stream()))
-        self.launches += 1 if self._body_out[1] is None else 2
+        self.launches += 1 if self._body_out[1] is None and self._ref_out == (None, None) else 2
         return out
 
     @property
@@ -311,6 +317,28 @@ class CudaEngine:
         self._body_out = (body, next_body)
         self.kernels_per_step = self.lib.locosim_kernels_per_step(self.h)     # (+1 while registered: body_kernel)
 
+    def set_reference_outputs(self, ref=None, next_ref=None):
+        """Register the reference outputs of include/locosim.h (the mocap clip's body outputs): `ref` and `next_ref` float32
+        cuda [n_envs, nbody, BODY_DIM], either None. A reference row is the body-output row of the state a reset onto the
+        table row at the env's cursor gives (root x / y zeroed; the rotation angle of the env's episode; its parameter-pool
+        row). Every step writes `ref` for the state `obs` describes (the cursor the terminal step reached for an env that
+        ended, zeros for a non-finite env) and `next_ref` for the state to act on next (after the auto-reset); reset() writes
+        `next_ref` as well, set_state() does not. The engine keeps a reference to them. None, None turns the feature off.
+        The CUDA-graph rules are those of set_body_outputs: register outside of capture and capture a step again after
+        turning the feature on."""
+        t = self.torch
+        shape = (self.n_envs, self.nbody, BODY_DIM)
+        for x, name in ((ref, "ref"), (next_ref, "next_ref")):
+            if x is None:
+                continue
+            if x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
+                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+            if tuple(x.shape) != shape:
+                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+        self._check(self.lib.locosim_set_reference_outputs(self.h, _ptr(ref), _ptr(next_ref)))
+        self._ref_out = (ref, next_ref)
+        self.kernels_per_step = self.lib.locosim_kernels_per_step(self.h)     # (+1 while registered: body_kernel)
+
     def set_contact_outputs(self, contact=None):
         """Register the contact outputs of include/locosim.h (MuJoCo's mj_contactForce summed per body): `contact` float32
         cuda [n_envs, nbody, CONTACT_DIM], or None to turn the feature off. Every step writes, per body, the world-frame force
@@ -368,6 +396,18 @@ class CudaEngine:
         self._check(self.lib.locosim_create_dataset(self.h, _ptr(states), _ptr(nxt), _ptr(last), self._stream()))
         self.launches += 1
         return states, nxt, last
+
+    def create_dataset_bodies(self):
+        """(body, next_body) float32 cuda [dataset rows, nbody, BODY_DIM], row-aligned with create_dataset(): the reference
+        rows of each row's (traj, sample) and (traj, sample + 1), with rotation angle 0 and the compiled model's own
+        parameters, built on the device."""
+        t = self.torch
+        n = self.lib.locosim_dataset_rows(self.h)
+        body = t.empty((n, self.nbody, BODY_DIM), dtype=t.float32, device=self.device)
+        nxt = t.empty_like(body)
+        self._check(self.lib.locosim_create_dataset_bodies(self.h, _ptr(body), _ptr(nxt), self._stream()))
+        self.launches += 1
+        return body, nxt
 
     def set_goal(self, goal):
         """goal: float32 cuda [n_envs, 4] per-episode goal features (A1: cos, sin, speed)."""

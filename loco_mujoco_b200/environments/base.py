@@ -245,6 +245,9 @@ class LocoEnv:
         self._contact_wrench = None
         # dof outputs (dof_outputs below): allocated and registered with the engine on first access
         self._dof_outputs = None
+        # reference outputs (reference_body_state / next_reference_body_state below): likewise
+        self._reference_body_state = None
+        self._next_reference_body_state = None
         self._engine = None
         self._obs = None
 
@@ -443,6 +446,8 @@ class LocoEnv:
                 self._engine.set_contact_outputs(self._contact_wrench)
             if self._dof_outputs is not None:
                 self._engine.set_dof_outputs(self._dof_outputs)
+            if self._reference_body_state is not None:
+                self._engine.set_reference_outputs(self._reference_body_state, self._next_reference_body_state)
         return self._engine
 
     # ---------------------------------------------------------------------------------------------------
@@ -566,6 +571,60 @@ class LocoEnv:
             eng.set_dof_outputs(t)
             self._dof_outputs = t
         return self._dof_outputs
+
+    # ---------------------------------------------------------------------------------------------------
+    # reference outputs (the mocap clip's body outputs, include/locosim.h locosim_set_reference_outputs)
+    # ---------------------------------------------------------------------------------------------------
+    @property
+    def reference_body_state(self):
+        """float32 torch tensor [num_envs, nbody, BODY_DIM = 13] on the env's device, rewritten by every step: the expert's
+        body state at each env's point in its mocap clip, in the layout and rows of `body_state`. A row is the `body_state`
+        row of the state that a reset onto the trajectory sample at the env's cursor would give: root x / y zeroed, the
+        rotation of the env's episode (setup_random_rot), the env's parameter-pool row. Right after a reset it equals
+        `next_body_state` bit for bit. Positions are root-x/y-relative: subtract the simulated root's x / y before comparing,
+        e.g. for foot row f and root row r
+            sim = body_state[:, f, :3].clone(); sim[:, :2] -= body_state[:, r, :2]
+            err = (sim - reference_body_state[:, f, :3]).norm(dim=-1)
+        It describes the state the step's observation describes: for an env that ended, the sample its terminal step
+        reached; zeros for an env whose state became non-finite. The cursor advances one sample per step only under
+        reward_type="tracking" or truncate_at_trajectory_end=True; with neither the reference would stay on the reset sample,
+        so this raises ValueError. Allocated and registered, together with `next_reference_body_state`, on first access of
+        either. Touch them before capturing a step in a CUDA graph (capture it again afterwards otherwise)."""
+        if self._reference_body_state is None:
+            self._new_reference_outputs()
+        return self._reference_body_state
+
+    @property
+    def next_reference_body_state(self):
+        """Like `reference_body_state`, for the state the env acts from next: after a step's auto-reset (rows of envs that
+        did not reset equal `reference_body_state`) and after reset(). reset(obs=...) moves no cursor and leaves it alone."""
+        if self._next_reference_body_state is None:
+            self._new_reference_outputs()
+        return self._next_reference_body_state
+
+    def _check_reference_phase(self):
+        if self._reward_type != "tracking" and not self._truncate_at_trajectory_end:
+            raise ValueError("the reference outputs follow the trajectory cursor, which advances only under "
+                             "reward_type=\"tracking\" or truncate_at_trajectory_end=True: make the env with one of them")
+
+    def _new_reference_outputs(self):
+        import torch
+        from ..engine import BODY_DIM
+        self._check_reference_phase()
+        eng = self._get_engine()
+        shape = (self.num_envs, self._model.nbody, BODY_DIM)
+        ref = torch.zeros(shape, dtype=torch.float32, device=eng.device)
+        nxt = torch.zeros(shape, dtype=torch.float32, device=eng.device)
+        eng.set_reference_outputs(ref, nxt)
+        self._reference_body_state, self._next_reference_body_state = ref, nxt
+
+    def create_dataset_bodies(self):
+        """The expert side of a body-space discriminator, built on the device: dict of float32 torch tensors body_states /
+        next_body_states [n, nbody, BODY_DIM], row-aligned with `create_dataset_device()` (states / next_states / last): row
+        r holds the body state of the reset onto dataset row r's trajectory sample, and of the next sample. Rotation angle
+        0, the compiled model's own parameters; positions root-x/y-relative as in `reference_body_state`."""
+        body, nxt = self._get_engine().create_dataset_bodies()
+        return dict(body_states=body, next_body_states=nxt)
 
     # ---------------------------------------------------------------------------------------------------
     # the hot path

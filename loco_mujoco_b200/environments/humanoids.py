@@ -322,6 +322,16 @@ class HumanoidTorque4AgesAll:
 
     dof_outputs = property(_no_dof_outputs)
 
+    # ---- reference outputs: likewise ----
+    def _no_reference_outputs(self, *args):
+        raise NotImplementedError("reference outputs (reference_body_state / next_reference_body_state / "
+                                  "create_dataset_bodies) are not available for HumanoidTorque4Ages mode 'all': use the "
+                                  "single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
+
+    reference_body_state = property(_no_reference_outputs)
+    next_reference_body_state = property(_no_reference_outputs)
+    create_dataset_bodies = _no_reference_outputs
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch

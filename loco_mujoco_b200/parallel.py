@@ -18,7 +18,8 @@ def shard_range(n_total, world_size, rank):
 
 def make_sharded(task_id, n_total, rank=None, world_size=None, device=None, seed=0, **kwargs):
     """LocoEnv for this rank's shard; `env_id_offset` keeps every env's random stream identical to the 1-GPU run.
-    Its `xfrc_applied` / `qfrc_applied`, `body_state` / `next_body_state`, `contact_wrench` and `dof_outputs` hold the rows of
+    Its `xfrc_applied` / `qfrc_applied`, `body_state` / `next_body_state`, `reference_body_state` /
+    `next_reference_body_state`, `contact_wrench` and `dof_outputs` hold the rows of
     this shard's envs only (global env offset + i is row i)."""
     from . import LocoEnv
     rank = dist.get_rank() if rank is None else rank
@@ -138,7 +139,8 @@ class MixedBatch:
     reach every member's engine. `step` returns the engines' own tuples, so `done` is the byte of include/locosim.h:
     `engine.split_done(done)` gives the absorbing and truncated masks, `engines[i].episode_stats()` the episode numbers.
     Applied forces are per member: `envs[i].xfrc_applied` / `envs[i].qfrc_applied` / `envs[i].body_index(name)`.
-    So are body outputs: `envs[i].body_state` / `envs[i].next_body_state`, contact outputs: `envs[i].contact_wrench`, and dof
+    So are body outputs: `envs[i].body_state` / `envs[i].next_body_state`, reference outputs:
+    `envs[i].reference_body_state` / `envs[i].next_reference_body_state`, contact outputs: `envs[i].contact_wrench`, and dof
     outputs: `envs[i].dof_outputs`.
     """
 
