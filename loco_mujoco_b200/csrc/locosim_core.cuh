@@ -182,7 +182,8 @@ __constant__ DevBodyOut c_bodyout[LS_MAX_SLOTS];  // (likewise)
 __constant__ DevContact c_contact[LS_MAX_SLOTS];  // (likewise)
 __constant__ int c_debug;      // diagnostic switches (LOCOSIM_DEBUG): 1 skip MPR, 2 skip the OBB filter, 4 drop convex pairs,
                                // 8 count MPR runs / support calls (locosim_debug_counters), 16 no separating-direction cache,
-                               // 32 no capsule-hull test of sphere | capsule | cylinder pairs
+                               // 32 no capsule-hull test of sphere | capsule | cylinder pairs, 64 primitive pairs in
+                               // rounds of 32 (filter, then narrow phase) also where C::PRIMLEAN
 __constant__ DevDof c_dof[LS_MAX_SLOTS];          // (a table of its own, like c_contact)
 // the dof outputs' [N, nu] scratch of the force per actuator, written by every dynamics evaluation while c_dof[ms].out is
 // registered (the actuator force is folded into qfrc_smooth, and the Euler state it was evaluated at is gone after the
@@ -201,9 +202,10 @@ enum {
   PH_EPILOGUE, PH_GROUPS,
   // collision() split: primitive filter rounds, primitive narrow phase + fill_contact, convex bounding-sphere loop, box (and
   // capsule-hull) tests, the job queue's first barrier, the warp's own jobs, the barrier that waits for the block's other
-  // jobs, convex_consume; then counts of the box-test survivors and of the jobs published
+  // jobs, convex_consume; then counts of the box-test survivors, of the jobs published, of the primitive pairs that pass
+  // the filter and of the primitive narrow sets (rounds) run
   PH_COL_PRIM_FILTER, PH_COL_PRIM_NARROW, PH_COL_SPHERES, PH_COL_OBB, PH_COL_QWAIT, PH_COL_JOBS, PH_COL_JOBS_WAIT,
-  PH_COL_CONSUME, PH_COL_NOBB, PH_COL_NJOBS, PH_N
+  PH_COL_CONSUME, PH_COL_NOBB, PH_COL_NJOBS, PH_COL_NPRIM, PH_COL_PRIM_SETS, PH_N
 };
 #if defined(LOCOSIM_PHASE_CLOCK) && !defined(LS_EMULATE)
 #define LS_PH_SLOTS (256 * 16)
@@ -1675,22 +1677,57 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
     }
   }
 #else
-  // 32 candidate pairs at a time: every lane filters its pair, the lanes that hit run the narrow phase in parallel,
-  // an exclusive scan over the lanes' contact counts assigns the slots, i.e. the list order is pair order, contact
-  // order within the pair: the same order as the serial loop (and as the oracle).
   const int lane = LS_LANE;
   // The pair table holds the primitive pairs first (ModelPack order: modelpack.pack partitions it), then the general convex
   // pairs: the latter only need the bounding-sphere test and a compaction, a lean loop (2 rounds of 32 per iteration).
   const int np_prim = m.np_prim;
   PH_T0(tc);
-  for (int base = 0; base < np_prim; base += 32) {
-    PH_LAP(PH_COL_PRIM_NARROW, tc);                     // (the previous round's narrow phase)
-    const int p = base + lane;
-    const int pk = p < np_prim ? e.pk_tab[p] : 0;
-    bool hit = (p < np_prim) && pair_filter(ms, e, p, pk);
-    const bool any = __any_sync(0xffffffffu, hit);
+  // C::PRIMLEAN: the primitive pairs get the same kind of lean loop (64 pairs per trip, both loads of a lane issued before
+  // either test), their hits are compacted in pair order into the candidate area (which the convex loop below only
+  // overwrites after the narrow sets have read it), and the narrow phase runs once per 32 hits (A1: its floor pairs in
+  // contact, one set). Otherwise, and with LOCOSIM_DEBUG bit 64: rounds of 32 pairs, the narrow phase after every round
+  // with a hit. Both give the same contact list. (`C::PRIMLEAN && lean` below, though `lean` implies it: so spelled, the
+  // lean code is gone before code generation in the other configurations, whose kernels keep the code they had.)
+  const bool lean = C::PRIMLEAN && !(c_debug & 64) && np_prim <= cand_max;
+  int nprim = 0;
+  if (C::PRIMLEAN && lean) {
+    NOUNROLL for (int base = 0; base < np_prim; base += 64) {
+      const int pa = base + lane, pb = pa + 32;
+      const int ka = pa < np_prim ? e.pk_tab[pa] : 0, kb = pb < np_prim ? e.pk_tab[pb] : 0;
+      const bool ha = pa < np_prim && pair_filter(ms, e, pa, ka);
+      const bool hb = pb < np_prim && pair_filter(ms, e, pb, kb);
+      const unsigned ma = __ballot_sync(0xffffffffu, ha), mb = __ballot_sync(0xffffffffu, hb);
+      if (ma | mb) {
+        const unsigned lt = (1u << lane) - 1u;
+        if (ha) cand[nprim + __popc(ma & lt)] = (unsigned short)pa;
+        if (hb) cand[nprim + __popc(ma) + __popc(mb & lt)] = (unsigned short)pb;
+        nprim += __popc(ma) + __popc(mb);
+      }
+    }
+    __syncwarp();
     PH_LAP(PH_COL_PRIM_FILTER, tc);
-    if (!any) continue;                                 // (most rounds of 32 pairs have no candidate at all)
+    PH_CNT(PH_COL_NPRIM, nprim);
+  }
+  // every set of 32: the lanes that hit run the narrow phase in parallel, an exclusive scan over the lanes' contact
+  // counts assigns the slots, i.e. the list order is pair order, contact order within the pair: the same order as the
+  // serial loop (and as the oracle)
+  for (int base = 0; base < (C::PRIMLEAN && lean ? nprim : np_prim); base += 32) {
+    PH_LAP(PH_COL_PRIM_NARROW, tc);                     // (the previous round's narrow phase)
+    int p;
+    bool hit;
+    if (C::PRIMLEAN && lean) {
+      hit = base + lane < nprim;
+      p = hit ? (int)cand[base + lane] : 0;
+    } else {
+      p = base + lane;
+      const int pk = p < np_prim ? e.pk_tab[p] : 0;
+      hit = (p < np_prim) && pair_filter(ms, e, p, pk);
+      const bool any = __any_sync(0xffffffffu, hit);
+      PH_LAP(PH_COL_PRIM_FILTER, tc);
+      if (!any) continue;                               // (most rounds of 32 pairs have no candidate at all)
+      PH_CNT(PH_COL_NPRIM, __popc(__ballot_sync(0xffffffffu, hit)));
+    }
+    PH_CNT(PH_COL_PRIM_SETS, 1);
     RawCon raw[4];
     int g1 = 0, g2 = 0, n = 0, nact = 0;
     float margin = 0, incl = 0;

@@ -28,10 +28,12 @@ PHASES = ["kinematics", "com_pos", "crb_factor", "smooth_forces", "collision", "
           "epilogue", "groups",
           # collision() split: primitive filter rounds, primitive narrow phase + fill_contact, convex bounding spheres, box
           # (and capsule-hull) tests, the job queue's first barrier, own jobs, the wait for the block's other jobs,
-          # convex_consume; counts of box-test survivors and of jobs published
+          # convex_consume; counts of box-test survivors, of jobs published, of primitive pairs that pass the filter and
+          # of primitive narrow sets (rounds) run
           "col_prim_filter", "col_prim_narrow", "col_spheres", "col_obb", "col_queue_wait", "col_jobs", "col_jobs_wait",
-          "col_consume", "col_obb_survivors", "col_jobs_published"]
-COUNTS = {"newton_trips", "newton_iters", "ls_evals", "substeps", "groups", "col_obb_survivors", "col_jobs_published"}
+          "col_consume", "col_obb_survivors", "col_jobs_published", "col_prim_candidates", "col_prim_sets"]
+COUNTS = {"newton_trips", "newton_iters", "ls_evals", "substeps", "groups", "col_obb_survivors", "col_jobs_published",
+          "col_prim_candidates", "col_prim_sets"}
 COLLISION_SPLIT = ["col_prim_filter", "col_prim_narrow", "col_spheres", "col_obb", "col_queue_wait", "col_jobs",
                    "col_jobs_wait", "col_consume"]
 
@@ -73,6 +75,8 @@ def table(raw):
         "collision_unsplit_cycles": cyc["collision"] - sum(cyc[k] for k in COLLISION_SPLIT),
         "convex_jobs_per_env_substep": c["col_jobs_published"] / n,
         "box_test_survivors_per_env_substep": c["col_obb_survivors"] / n,
+        "primitive_candidates_per_env_substep": c["col_prim_candidates"] / n,
+        "primitive_narrow_sets_per_env_substep": c["col_prim_sets"] / n,
         "env_substeps": c["substeps"], "groups": c["groups"],
         "prologue_epilogue_cycles_per_group": (c["prologue"] + c["epilogue"]) / max(1, c["groups"]),
     }
