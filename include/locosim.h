@@ -200,6 +200,8 @@ int locosim_set_contact_outputs(locosim_t* h, float* d_contact);
  *   1 qfrc_constraint  J^T efc_force at the solver's final qacc, as mj_fwdConstraint leaves it
  *   2 qacc             the constrained acceleration of mj_forward. For the Euler integrator this is NOT the solve with
  *                      implicit joint damping that the integrator advances with (which MuJoCo also keeps out of d->qacc).
+ *                      locosim_inverse below is the continuous-time inverse of this qacc; MuJoCo 3's discrete-time inverse
+ *                      (mjENBL_INVDISCRETE), which would invert the implicit-damping solve, is not built.
  * Time window: the MEAN over the control step's sub-steps; each sub-step contributes its last dynamics evaluation (Euler: its
  * only one; RK4: its fourth stage), the window of the contact outputs. This differs from MuJoCo's mjData after mj_step, which
  * holds the last sub-step only, evaluated at that sub-step's START state (RK4: its first stage).
@@ -251,6 +253,37 @@ int locosim_set_reference_outputs(locosim_t* h, float* d_ref, float* d_next_ref)
  * (traj, sample + 1) in d_next_body, with rotation angle 0 and the compiled model's own parameters (what an env runs with when
  * no parameter pool is set). Stream-ordered; the expert side of a body-space discriminator. */
 int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_body, void* stream);
+
+/* Inverse dynamics, MuJoCo 2.3.7's continuous-time mj_inverse: the generalised force that produces a given acceleration at
+ * a given state, contacts included. For an env with state (qpos, qvel), its parameter-pool row and an acceleration qacc:
+ *   qfrc_inverse = M(q) qacc + qfrc_bias(q, v) - qfrc_passive(q, v) - qfrc_constraint(q, v, qacc)
+ * with M including dof_armature, qfrc_bias the RNE bias with gravity, qfrc_passive the joint stiffness plus the explicit
+ * damping -b qvel, and qfrc_constraint = J^T efc_force, efc_force the soft-constraint force of jar = J qacc - aref (the
+ * solver's map, mj_constraintUpdate): friction loss, joint limits and contacts (the configuration's cone), over the
+ * contact set the state gives, with the per-env row cap of the forward dynamics. Actuator forces, qfrc_applied and
+ * xfrc_applied are NOT subtracted, as in MuJoCo, so at a forward solution
+ *   qfrc_inverse ~= qfrc_actuator + qfrc_applied + J^T xfrc_applied     (up to the solver's convergence: mjENBL_FWDINV)
+ * and registered applied forces change no bit of the result. The integrator plays no part (continuous time).
+ * A non-finite qpos, qvel or qacc of an env gives that env a row of zeros (and that state reaches no collision test).
+ * The call reads the state and changes nothing else: state, warm start, counters, cursors, random streams, episode
+ * statistics and every registered output stay as they were.
+ *
+ * locosim_inverse: every env at its stored state (what locosim_get_state returns) and its current pool row (carry tasks:
+ * the carried weight's model). d_qacc, d_qfrc_inverse fp32 [n_envs, nv] DEVICE buffers in the qvel dof order of
+ * locosim_get_state and qfrc_applied (every in-scope model has nq == nv); they must not overlap (refused). Stream-ordered,
+ * no host synchronisation, no allocation: it can be captured in a CUDA graph (a replay reads the buffers and the state as
+ * they are then). */
+int locosim_inverse(locosim_t* h, const float* d_qacc, float* d_qfrc_inverse, void* stream);
+
+/* Inverse dynamics of the whole dataset, row-aligned with locosim_create_dataset and locosim_create_dataset_bodies:
+ * d_qfrc fp32 [locosim_dataset_rows, nv]. Row r, (traj, sample) -> (traj, sample + 1), is the inverse at the reset state of
+ * (traj, sample) (reset_value with rotation angle 0 and the compiled model's own parameters, as the dataset's reference
+ * rows) at the forward-difference acceleration of the dataset's control rate, exactly
+ *   inv_dt = (float)(1.0 / ((double)timestep * n_substeps))       (timestep: the model's fp32 timestep, on the host)
+ *   qacc   = (qvel[sample + 1] - qvel[sample]) * inv_dt           (fp32, qvel as reset_value gives it)
+ * so that a caller can rebuild qacc bit for bit. Stream-ordered: the forces a mocap clip needs, and the residual on the
+ * unactuated root dofs. */
+int locosim_create_dataset_inverse(locosim_t* h, float* d_qfrc, void* stream);
 
 /* Per-episode goal features (UnitreeA1: cos / sin of the goal direction and the goal speed, GoalDirectionVelocity set in
  * setup() unitreeA1.py:287-291); normally loaded from the reset table, settable for reset(obs=...) (base.py:217-218,633-654).

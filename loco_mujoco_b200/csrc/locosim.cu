@@ -952,6 +952,68 @@ __global__ void __launch_bounds__(32) dataset_body_kernel(int ms, DevTask t, con
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// Inverse dynamics (locosim_inverse, locosim_create_dataset_inverse), one warp and one EnvS per block, the pair table read
+// from global memory. EnvS::substep = -1: no output hook of the stages stores anything. The engine's state, counters and
+// outputs are only read.
+// ----------------------------------------------------------------------------------------------------------
+// pk: the handle's staged pair table in global memory (the source of the step kernels' TMA copy, whose layout DevModel::pk_n
+// then describes), or NULL: the model's table
+template <class C>
+LS_DEV void inverse_setup(const int ms, EnvS<C>& e, const float* prm, const int env, const int* pk) {
+  if ((threadIdx.x & 31) == 0) {
+    e.prm = prm;
+    e.pk_tab = pk ? pk : c_models[ms].pair_packed;
+    e.env = env;
+    e.substep = -1;
+  }
+  __syncwarp();
+  init_workspace(ms, e);
+}
+
+// reset_value's qvel at rotation angle 0, with sin 0 = 0 and cos 0 = 1 spelled out: the same bits without sincosf
+__device__ __forceinline__ float reset_qvel0(const DevTask& t, const float* row, int nv, int idx) {
+  if (t.rot[0] >= 0 && (idx == t.rot[1] || idx == t.rot[2])) {
+    const float vx = row[nv + t.rot[1]], vy = row[nv + t.rot[2]];
+    return idx == t.rot[1] ? 1.0f * vx - 0.0f * vy : 0.0f * vx + 1.0f * vy;
+  }
+  return row[nv + idx];
+}
+
+// One kernel for both calls, one warp and one EnvS per block, the pair table read from global memory (no TMA staging).
+//   inv_dt == 0 (locosim_inverse): block = env, at its stored state and parameter-pool row: qacc / qfrc [n_envs, nv]
+//   inv_dt > 0 (locosim_create_dataset_inverse): block = row r of locosim_create_dataset, (traj, sample) -> (traj,
+//     sample + 1): the reset state of (traj, sample) (angle 0, parameters `prm`, the compiled model's own) at
+//     qacc = (qvel[sample + 1] - qvel[sample]) * inv_dt; qfrc [rows, nv]
+template <class C>
+__global__ void __launch_bounds__(32) inverse_kernel(int ms, EngineState st, DevTask t, const int* __restrict__ pk,
+                                                     const float* __restrict__ qacc, const float* __restrict__ prm, float inv_dt,
+                                                     float* __restrict__ qfrc) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  EnvS<C>& e = *reinterpret_cast<EnvS<C>*>(smem_raw);
+  const DevModel& m = c_models[ms];
+  const int r = blockIdx.x, lane = threadIdx.x & 31, nv = m.nv;
+  if (inv_dt > 0.0f) {
+    const int per = t.traj_len - 1, tj = r / per, sp = r - tj * per, ncol = 2 * nv + t.n_goal;
+    const float* row = t.table + ((size_t)tj * t.traj_len + sp) * ncol;
+    inverse_setup(ms, e, prm, r, pk);
+    for (int i = lane; i < nv; i += 32) {
+      e.qpos[i] = reset_value(t, row, nv, LS_OBS_QPOS, i, 0.0f);
+      e.qvel[i] = reset_qvel0(t, row, nv, i);
+      e.qacc[i] = (reset_qvel0(t, row + ncol, nv, i) - e.qvel[i]) * inv_dt;
+    }
+  } else {
+    inverse_setup(ms, e, st.pool + (size_t)st.dr_row[r] * m.pool_P, r, pk);
+    for (int i = lane; i < nv; i += 32) {
+      e.qpos[i] = st.qpos[(size_t)r * nv + i];
+      e.qvel[i] = st.qvel[(size_t)r * nv + i];
+      e.qacc[i] = qacc[(size_t)r * nv + i];
+    }
+  }
+  __syncwarp();
+  inverse_dynamics(ms, e, qfrc + (size_t)r * nv);
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // Regrouping: the warps of a block run the solver in lock-step, so a block is as slow as its hardest env. Solver effort
 // is strongly correlated from one control step to the next (lag-1 correlation of the per-step Newton iteration count
 // ~0.6), so before every step the envs are bucketed by the iteration count of their previous step (counting sort,
@@ -1050,6 +1112,35 @@ static int launch_dataset_bodies(locosim_handle* h, float* body, float* next_bod
   const int rows = h->ht.n_traj * (h->ht.traj_len - 1);
   if (rows > 0)
     dataset_body_kernel<C><<<rows, 32, sizeof(EnvS<C>), s>>>(h->slot, h->dt, h->d_model_row, body, next_body);
+  CK(cudaGetLastError());
+  return 0;
+}
+// C with the primitive pairs filtered by collision()'s round loop (PRIMLEAN = 0: the same contact list as the lean pass, and
+// the same EnvS layout). inverse_kernel is instantiated with it in every configuration, so that it compiles to the same
+// registers and stack whichever pass UnitreeA1's step kernels use (LOCOSIM_PRIMLEAN), and its stages are copies of their
+// own that leave the step kernels' untouched.
+template <class C>
+struct RoundLoop : C { enum { PRIMLEAN = 0 }; };
+template <class C>
+static int launch_inverse(locosim_handle* h, const float* qacc, float* qfrc, cudaStream_t s) {
+  static_assert(sizeof(EnvS<C>) <= 48 * 1024, "inverse_kernel: one EnvS per block within the default shared-memory limit");
+  inverse_kernel<RoundLoop<C>><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, h->dt, (const int*)h->d_stage,
+                                                                       qacc, nullptr, 0.0f, qfrc);
+  CK(cudaGetLastError());
+  return 0;
+}
+// 1 / (timestep * n_substeps), the dataset's control rate, in double from the model's fp32 timestep (the device code divides
+// with -prec-div=false; a caller rebuilds the dataset's qacc bit for bit from this value)
+static float dataset_inv_dt(const locosim_handle* h) {
+  return (float)(1.0 / ((double)h->hm.timestep * (double)h->dt.n_substeps));
+}
+template <class C>
+static int launch_dataset_inverse(locosim_handle* h, float* qfrc, cudaStream_t s) {
+  static_assert(sizeof(EnvS<C>) <= 48 * 1024, "inverse_kernel: one EnvS per block within the default shared-memory limit");
+  const int rows = h->ht.n_traj * (h->ht.traj_len - 1);
+  if (rows > 0)
+    inverse_kernel<RoundLoop<C>><<<rows, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, h->dt, (const int*)h->d_stage,
+                                                                   nullptr, h->d_model_row, dataset_inv_dt(h), qfrc);
   CK(cudaGetLastError());
   return 0;
 }
@@ -1242,6 +1333,9 @@ extern "C" int locosim_configs31_sync_model(locosim_handle* h) __attribute__((we
 extern "C" int locosim_configs31_body(locosim_handle* h, const uint8_t* mask, int parts, cudaStream_t s) __attribute__((weak));
 extern "C" int locosim_configs31_dataset_bodies(locosim_handle* h, float* body, float* next_body, cudaStream_t s)
     __attribute__((weak));
+extern "C" int locosim_configs31_inverse(locosim_handle* h, const float* qacc, float* qfrc, cudaStream_t s)
+    __attribute__((weak));
+extern "C" int locosim_configs31_dataset_inverse(locosim_handle* h, float* qfrc, cudaStream_t s) __attribute__((weak));
 
 // body_kernel outside a step, for the envs of `mask` (NULL = all), the parts (see body_kernel) that are registered:
 // d_next_body (1) after locosim_reset* and locosim_set_state; the reference keys (2) and d_next_ref (4) after locosim_reset*,
@@ -1433,13 +1527,18 @@ int locosim_set_reference_outputs(locosim_t* h, float* d_ref, float* d_next_ref)
   CK(cudaDeviceSynchronize());
   return 0;
 }
-int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_body, void* stream) {
-  if (!d_body || !d_next_body) { h->err = "null buffer"; return 1; }
-  CK(cudaSetDevice(h->device));
+// the compiled model's own parameter row on the device (h->d_model_row), uploaded on first use
+static int model_row(locosim_handle* h) {
   if (!h->d_model_row) {
     CK(cudaMalloc((void**)&h->d_model_row, h->hm.default_row.size() * 4));
     CK(cudaMemcpy(h->d_model_row, h->hm.default_row.data(), h->hm.default_row.size() * 4, cudaMemcpyHostToDevice));
   }
+  return 0;
+}
+int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_body, void* stream) {
+  if (!d_body || !d_next_body) { h->err = "null buffer"; return 1; }
+  CK(cudaSetDevice(h->device));
+  if (model_row(h)) return 1;
   cudaStream_t s = (cudaStream_t)stream;
   switch (h->cfg) {
     case 0: return launch_dataset_bodies<CfgEllEuler>(h, d_body, d_next_body, s);
@@ -1448,6 +1547,36 @@ int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_bod
     case 4:
     case 5: return locosim_configs31_dataset_bodies(h, d_body, d_next_body, s);
     default: return launch_dataset_bodies<CfgPyrRK4>(h, d_body, d_next_body, s);
+  }
+}
+int locosim_inverse(locosim_t* h, const float* d_qacc, float* d_qfrc_inverse, void* stream) {
+  if (!d_qacc || !d_qfrc_inverse) { h->err = "null buffer"; return 1; }
+  const size_t bytes = (size_t)h->n_envs * h->hm.nv * 4;
+  const char *a = (const char*)d_qacc, *b = (const char*)d_qfrc_inverse;
+  if (a < b + bytes && b < a + bytes) { h->err = "qacc and qfrc_inverse overlap"; return 1; }
+  CK(cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (h->cfg) {
+    case 0: return launch_inverse<CfgEllEuler>(h, d_qacc, d_qfrc_inverse, s);
+    case 1: return launch_inverse<CfgPyrEuler>(h, d_qacc, d_qfrc_inverse, s);
+    case 3: return launch_inverse<CfgPyrEuler29>(h, d_qacc, d_qfrc_inverse, s);
+    case 4:
+    case 5: return locosim_configs31_inverse(h, d_qacc, d_qfrc_inverse, s);
+    default: return launch_inverse<CfgPyrRK4>(h, d_qacc, d_qfrc_inverse, s);
+  }
+}
+int locosim_create_dataset_inverse(locosim_t* h, float* d_qfrc, void* stream) {
+  if (!d_qfrc) { h->err = "null buffer"; return 1; }
+  CK(cudaSetDevice(h->device));
+  if (model_row(h)) return 1;
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (h->cfg) {
+    case 0: return launch_dataset_inverse<CfgEllEuler>(h, d_qfrc, s);
+    case 1: return launch_dataset_inverse<CfgPyrEuler>(h, d_qfrc, s);
+    case 3: return launch_dataset_inverse<CfgPyrEuler29>(h, d_qfrc, s);
+    case 4:
+    case 5: return locosim_configs31_dataset_inverse(h, d_qfrc, s);
+    default: return launch_dataset_inverse<CfgPyrRK4>(h, d_qfrc, s);
   }
 }
 int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {

@@ -86,4 +86,22 @@ int locosim_configs31_dataset_bodies(Handle31* h, float* body, float* next_body,
   }
 }
 
+int locosim_configs31_inverse(Handle31* h, const float* qacc, float* qfrc, cudaStream_t s) {
+  using namespace locosim31;
+  switch (h->cfg) {
+    case 4: return launch_inverse<CfgPyrRK4_31>(h, qacc, qfrc, s);
+    case 5: return launch_inverse<CfgPyrEuler31>(h, qacc, qfrc, s);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
+int locosim_configs31_dataset_inverse(Handle31* h, float* qfrc, cudaStream_t s) {
+  using namespace locosim31;
+  switch (h->cfg) {
+    case 4: return launch_dataset_inverse<CfgPyrRK4_31>(h, qfrc, s);
+    case 5: return launch_dataset_inverse<CfgPyrEuler31>(h, qfrc, s);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
 }

@@ -2842,6 +2842,109 @@ LS_FN void forward(const int ms, EnvS<C>& e, const SolverOpts so) {
   fwd_constraint(ms, e, so);
 }
 
+// ----------------------------------------------------------------------------------------------------------
+// inverse dynamics (locosim_inverse): MuJoCo 2.3.7's continuous-time mj_inverse
+// ----------------------------------------------------------------------------------------------------------
+// qfrc_smooth = passive - bias: passes (A) - (C) of smooth_forces without the applied and actuator forces, which mj_inverse
+// does not subtract. Kept apart from smooth_forces, whose code the step kernels must keep unchanged; qfrc_smooth lies
+// outside the storage that collision() and make_constraint() overwrite.
+template <class C>
+LS_FN void passive_bias(const int ms, EnvS<C>& e) {
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv;
+  PAR_FOR(j, nv) {
+    unsigned mask = (unsigned)m.body_dofmask[m.jnt_bodyid[j]] & ((1u << j) - 1u);
+    float v[6] = {0, 0, 0, 0, 0, 0};
+    while (mask) {
+      const int i = LS_FFS(mask) - 1;
+      mask &= mask - 1;
+      const float qv = e.qvel[i];
+      for (int c = 0; c < 6; c++) v[c] = fmaf(e.cdof[i][c], qv, v[c]);
+    }
+    float cdd[6];
+    crossMotion(cdd, v, e.cdof[j]);
+    for (int c = 0; c < 6; c++) e.cdof_dot[j][c] = cdd[c];
+  }
+  SYNC();
+  PAR_FOR(b, m.nb) {
+    float* f = e.crb[b];
+    if (b == 0) { for (int k = 0; k < 6; k++) f[k] = 0; continue; }
+    unsigned mask = (unsigned)m.body_dofmask[b];
+    float cvel[6] = {0, 0, 0, 0, 0, 0}, cacc[6] = {0, 0, 0, -m.gravity[0], -m.gravity[1], -m.gravity[2]};
+    while (mask) {
+      const int i = LS_FFS(mask) - 1;
+      mask &= mask - 1;
+      const float qv = e.qvel[i];
+      for (int c = 0; c < 6; c++) { cvel[c] = fmaf(e.cdof[i][c], qv, cvel[c]); cacc[c] = fmaf(e.cdof_dot[i][c], qv, cacc[c]); }
+    }
+    float t1[6], t2[6], t3[6];
+    mulInertVec(t1, e.cinert[b], cacc);
+    mulInertVec(t2, e.cinert[b], cvel);
+    crossForce(t3, cvel, t2);
+    for (int k = 0; k < 6; k++) f[k] = t1[k] + t3[k];
+  }
+  SYNC();
+  PAR_FOR(j, nv) {
+    float F[6] = {0, 0, 0, 0, 0, 0};
+    NOUNROLL for (int b = 1; b < m.nb; b++) {
+      if (!((m.body_dofmask[b] >> j) & 1)) continue;
+      for (int c = 0; c < 6; c++) F[c] += e.crb[b][c];
+    }
+    float bias = 0;
+    for (int c = 0; c < 6; c++) bias += e.cdof[j][c] * F[c];
+    float passive = -PRM(jnt_stiffness)[j] * (e.qpos[j] - m.qpos_spring[j]) - PRM(dof_damping)[j] * e.qvel[j];
+    e.qfrc_smooth[j] = passive - bias;
+  }
+  SYNC();
+}
+
+// qfrc_inverse = M qacc + bias - passive - J^T efc_force into out[0, nv), for the state e.qpos / e.qvel, the acceleration
+// e.qacc and the parameters e.prm (the caller has run init_workspace; entries >= nv of e.qacc are 0). efc_force is the
+// solver's soft-constraint map (constraint_update) of jar = J qacc - aref over the rows the state gives: the contact set
+// of collision() and the row cap of make_constraint(), as in forward(). A non-finite qpos, qvel or qacc gives a row of
+// zeros before anything reaches collision(). A whole-warp call; it writes nothing but out and the env's working set.
+template <class C>
+LS_FN void inverse_dynamics(const int ms, EnvS<C>& e, float* out) {
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv;
+  bool bad = false;
+  PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]) && isfinite(e.qacc[i]));
+#ifndef LS_EMULATE
+  bad = __any_sync(0xffffffffu, bad);
+#endif
+  if (bad) {
+    PAR_FOR(i, nv) out[i] = 0.0f;
+    SYNC();
+    return;
+  }
+  kinematics(ms, e);
+  com_pos(ms, e);
+  crb_factor(ms, e);
+  passive_bias(ms, e);         // (before collision: the constraint rows overlay the scratch it reads)
+  collision(ms, e);
+  make_constraint(ms, e);
+  const int nefc = e.nefc, nunit = e.nunit, nrow = e.nrow;
+  mulJ(ms, e, e.r_jar, e.qacc);
+  SYNC();
+  PAR_FOR(r, nefc) e.r_jar[r] -= e.r_aref[r];
+  SYNC();
+  constraint_update(ms, e);
+  mulM(ms, e, e.Ma, e.qacc);
+  SYNC();
+  // J^T efc_force in finish_constraint's order (its Gauss term reads qacc_smooth, which this path does not compute)
+  PAR_FOR(d, nv) {
+    float a = 0;
+    const int fr = m.dof_frow[d];
+    if (fr >= 0) a += e.r_force[fr];
+    const int l0 = e.d_lrow[d][0], l1 = e.d_lrow[d][1];
+    if (l0 >= 0) a += e.r_force[l0];
+    if (l1 >= 0) a -= e.r_force[l1];
+    for (int r = 0; r < nrow; r++) a = fmaf(e.J[r][d], e.r_force[nunit + r], a);
+    out[d] = e.Ma[d] - e.qfrc_smooth[d] - a;
+  }
+  SYNC();
+}
+
 template <class C>
 LS_FN void euler_step(const int ms, EnvS<C>& e) {
   const DevModel& m = c_models[ms];

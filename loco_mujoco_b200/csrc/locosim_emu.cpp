@@ -31,6 +31,7 @@ struct EmuBase {
   virtual void poison() = 0;
   virtual void body(float* out) = 0;
   virtual void ref(const DevTask& t, const float* row, float angle, float* out) = 0;
+  virtual void inv(const double* qacc, float* out) = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -96,6 +97,12 @@ struct EmuT : EmuBase {
     c_models[0] = m;
     reference_outputs(0, t, e, row, angle, out, (float*)nullptr);
   }
+  void inv(const double* qacc, float* out) override {
+    c_models[0] = m;
+    e.substep = -1;
+    for (int i = 0; i < m.nv; i++) e.qacc[i] = (float)qacc[i];
+    inverse_dynamics(0, e, out);
+  }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
 
@@ -153,6 +160,10 @@ void emu_reference_row(EmuBase* s, const float* row, const int* recenter, const 
   for (int k = 0; k < 3; k++) t.rot[k] = rot ? rot[k] : -1;
   s->ref(t, row, angle, out);
 }
+// inverse dynamics (locosim_inverse) of the emulated env's current state at the acceleration qacc [nv]: fp32 [nv] into `out`,
+// with the model's own parameters. Overwrites the env's acceleration and constraint working set (not its state or warm
+// start), as a forward evaluation would.
+void emu_inverse(EmuBase* s, const double* qacc, float* out) { s->inv(qacc, out); }
 // contact outputs of the emulated env (locosim_set_contact_outputs; row 0 of the engine's layout: fp32 [nb, LS_CONTACT_DIM], or
 // NULL): every later emu_step(ctrl, nsub) runs as one control step of nsub sub-steps and leaves their mean wrench there
 void emu_set_contact(EmuBase* s, float* wrench) { s->cw.wrench = wrench; }

@@ -92,6 +92,10 @@ def load_library():
     lib.locosim_set_reference_outputs.argtypes = [vp, vp, vp]
     lib.locosim_create_dataset_bodies.restype = ip
     lib.locosim_create_dataset_bodies.argtypes = [vp, vp, vp, vp]
+    lib.locosim_inverse.restype = ip
+    lib.locosim_inverse.argtypes = [vp, vp, vp, vp]
+    lib.locosim_create_dataset_inverse.restype = ip
+    lib.locosim_create_dataset_inverse.argtypes = [vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -105,7 +109,8 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_debug_counters", "locosim_set_timeline", "locosim_set_time_limit",
                     "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
                     "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs",
-                    "locosim_set_reference_outputs", "locosim_create_dataset_bodies"]
+                    "locosim_set_reference_outputs", "locosim_create_dataset_bodies", "locosim_inverse",
+                    "locosim_create_dataset_inverse"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -408,6 +413,41 @@ class CudaEngine:
         self._check(self.lib.locosim_create_dataset_bodies(self.h, _ptr(body), _ptr(nxt), self._stream()))
         self.launches += 1
         return body, nxt
+
+    def inverse(self, qacc, out=None):
+        """Inverse dynamics of include/locosim.h (MuJoCo 2.3.7's continuous-time mj_inverse) of every env at its stored
+        state and parameter-pool row: qfrc_inverse = M qacc + bias - passive - J^T efc_force(J qacc - aref), actuator and
+        applied forces not subtracted. `qacc` float32 cuda [n_envs, nq] (the qvel layout); `out` float32 cuda [n_envs, nq]
+        not overlapping it, or None for a new tensor. A non-finite state or qacc gives that env a row of zeros. Changes
+        nothing else in the engine; stream-ordered, no allocation when `out` is given (can be captured in a CUDA graph)."""
+        t = self.torch
+        shape = (self.n_envs, self.nq)
+        if out is None:
+            out = t.empty(shape, dtype=t.float32, device=self.device)
+        for x, name in ((qacc, "qacc"), (out, "out")):
+            if not isinstance(x, t.Tensor) or x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
+                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+            if tuple(x.shape) != shape:
+                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+        nbytes = self.n_envs * self.nq * 4
+        a, b = qacc.data_ptr(), out.data_ptr()
+        if a < b + nbytes and b < a + nbytes:
+            raise ValueError("qacc and out must not overlap")
+        self._check(self.lib.locosim_inverse(self.h, _ptr(qacc), _ptr(out), self._stream()))
+        self.launches += 1
+        return out
+
+    def create_dataset_inverse(self):
+        """float32 cuda [dataset rows, nq], row-aligned with create_dataset(): row r is the inverse dynamics at the reset
+        state of its (traj, sample) (rotation angle 0, the compiled model's own parameters) at the forward-difference
+        acceleration qacc = (qvel[sample + 1] - qvel[sample]) * inv_dt, inv_dt = float32(1 / (timestep * n_substeps))
+        computed in double from the model's float32 timestep. Built on the device."""
+        t = self.torch
+        n = self.lib.locosim_dataset_rows(self.h)
+        out = t.empty((n, self.nq), dtype=t.float32, device=self.device)
+        self._check(self.lib.locosim_create_dataset_inverse(self.h, _ptr(out), self._stream()))
+        self.launches += 1
+        return out
 
     def set_goal(self, goal):
         """goal: float32 cuda [n_envs, 4] per-episode goal features (A1: cos, sin, speed)."""

@@ -627,6 +627,43 @@ class LocoEnv:
         return dict(body_states=body, next_body_states=nxt)
 
     # ---------------------------------------------------------------------------------------------------
+    # inverse dynamics (MuJoCo's mj_inverse, include/locosim.h locosim_inverse)
+    # ---------------------------------------------------------------------------------------------------
+    def dof_index(self, joint_name):
+        """Column of joint `joint_name`'s dof in `qfrc_applied`, `dof_outputs`, `inverse_dynamics()` and
+        `create_dataset_inverse()` (every model here has one dof per joint, in the qvel order of the state). ValueError for
+        an unknown name."""
+        names = list(self._model.jnt_names)
+        if joint_name not in names:
+            raise ValueError("no joint %r in the model (joints: %s)" % (joint_name, ", ".join(names)))
+        return names.index(joint_name)
+
+    def inverse_dynamics(self, qacc):
+        """MuJoCo's mj_inverse (2.3.7, continuous time) of every env at its current state, the state of info["next_obs"]
+        (the one the env acts from next), with its parameter-pool row: float32 torch tensor [num_envs, nq] on the env's
+        device,
+            qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint(qacc)
+        where qfrc_constraint is J^T of the soft-constraint forces that `qacc` implies at the state (contacts, joint limits,
+        friction loss). Actuator forces, `qfrc_applied` and `xfrc_applied` are not subtracted, so at the engine's own
+        forward solution it is the actuator force plus the applied forces (the root dofs' entries: the "hand of god" force
+        a motion needs). `qacc`: float32 [num_envs, nq] on the env's device, in the qvel layout (`dof_index`). A non-finite
+        state or qacc gives that env a row of zeros. Changes nothing in the env."""
+        import torch
+        eng = self._get_engine()
+        if not isinstance(qacc, torch.Tensor):
+            raise ValueError("qacc must be a float32 torch tensor [num_envs, nq] on %s" % eng.device)
+        return eng.inverse(qacc)
+
+    def create_dataset_inverse(self):
+        """The joint-space forces the mocap clip needs, built on the device: float32 torch tensor [n, nq], row-aligned with
+        `create_dataset_device()` and `create_dataset_bodies()`. Row r is `inverse_dynamics` at the reset state of dataset
+        row r's trajectory sample (rotation angle 0, the compiled model's own parameters) at the forward-difference
+        acceleration to the next sample, qacc = (qvel[next] - qvel) * float32(1 / (timestep * n_substeps)). Columns of
+        actuated joints hold the torque the clip requires; those of the unactuated root dofs, the residual force that
+        measures how physically consistent the clip is on this robot."""
+        return self._get_engine().create_dataset_inverse()
+
+    # ---------------------------------------------------------------------------------------------------
     # the hot path
     # ---------------------------------------------------------------------------------------------------
     def reward(self, state, action, next_state, absorbing):

@@ -332,6 +332,16 @@ class HumanoidTorque4AgesAll:
     next_reference_body_state = property(_no_reference_outputs)
     create_dataset_bodies = _no_reference_outputs
 
+    # ---- inverse dynamics: likewise ----
+    def _no_inverse_dynamics(self, *args):
+        raise NotImplementedError("inverse dynamics (inverse_dynamics / create_dataset_inverse / dof_index) is not available "
+                                  "for HumanoidTorque4Ages mode 'all': use the single-scaling envs "
+                                  "(HumanoidTorque4Ages.<task>.<1-4>)")
+
+    inverse_dynamics = _no_inverse_dynamics
+    create_dataset_inverse = _no_inverse_dynamics
+    dof_index = _no_inverse_dynamics
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch
