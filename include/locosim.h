@@ -285,6 +285,31 @@ int locosim_inverse(locosim_t* h, const float* d_qacc, float* d_qfrc_inverse, vo
  * unactuated root dofs. */
 int locosim_create_dataset_inverse(locosim_t* h, float* d_qfrc, void* stream);
 
+/* Model-based dynamics terms of every env at its stored state (what locosim_get_state returns, the state of
+ * info["next_obs"]) with its current parameter-pool row (carry tasks: the carried weight's model), in MuJoCo 2.3.7's
+ * meaning. All outputs are fp32 DEVICE buffers, env-major; dofs in the qvel order of locosim_get_state (every in-scope
+ * model has nq == nv), body rows in the compiled model's body indices (those of xfrc_applied and the body outputs):
+ *   d_M        [n_envs, nv, nv]         mj_fullM of d->qM: dense, symmetric, dof_armature on the diagonal
+ *   d_bias     [n_envs, nv]             d->qfrc_bias: mj_rne with qacc = 0 (Coriolis, centrifugal and gravity)
+ *   d_passive  [n_envs, nv]             d->qfrc_passive: -stiffness (q - q_spring) - damping qvel, the term locosim_inverse
+ *                                       subtracts
+ *   d_com      [n_envs, LS_COM_DIM]     the whole-robot centre of mass d->subtree_com[0] (x, y, z), then the total mass; a
+ *                                       carried weight is part of the robot, and both follow the env's pool row
+ *   d_jac      [n_envs, nbody, 6, nv]   per body, rows 0-2 jacr and rows 3-5 jacp of mj_jacBody: the Jacobian of the
+ *                                       body-frame origin xpos (NOT xipos) in world coordinates, rows in body_state's order
+ *                                       (angular, then linear velocity), so jac[i, b] @ qvel[i] = body_state[i, b, 7:13];
+ *                                       body 0 (the world) is all zeros. xfrc_applied acts at xipos, so J^T F with this
+ *                                       Jacobian is NOT the generalised force of an xfrc_applied force.
+ *   d_jac_com  [n_envs, 3, nv]          mj_jacSubtreeCom of the whole robot: d(com) / dq, i.e. com velocity = jac_com qvel
+ * Any output may be NULL; with all six NULL the call launches nothing and returns 0. Overlapping outputs are refused.
+ * A non-finite qpos or qvel of an env gives that env zero rows in every output. The call reads the state and changes
+ * nothing else: state, warm start, counters, cursors, random streams, episode statistics and every registered output stay
+ * as they were. Stream-ordered, no host synchronisation, no allocation: it can be captured in a CUDA graph (a replay reads
+ * the state as it is then). */
+#define LS_COM_DIM 4
+int locosim_dynamics_terms(locosim_t* h, float* d_M, float* d_bias, float* d_passive, float* d_com, float* d_jac,
+                           float* d_jac_com, void* stream);
+
 /* Per-episode goal features (UnitreeA1: cos / sin of the goal direction and the goal speed, GoalDirectionVelocity set in
  * setup() unitreeA1.py:287-291); normally loaded from the reset table, settable for reset(obs=...) (base.py:217-218,633-654).
  * d_goal fp32 [n_envs, 4]. */

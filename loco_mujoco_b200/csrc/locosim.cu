@@ -1014,6 +1014,34 @@ __global__ void __launch_bounds__(32) inverse_kernel(int ms, EngineState st, Dev
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// Dynamics terms (locosim_dynamics_terms), inverse_kernel's layout: one warp and one EnvS per block (block = env), at the
+// env's stored state and parameter-pool row. No collision runs, so no pair table is read. EnvS::substep = -1; the engine's
+// state, counters and outputs are only read. `o` holds the whole buffers (or NULL); each env writes its own rows.
+// ----------------------------------------------------------------------------------------------------------
+template <class C>
+__global__ void __launch_bounds__(32) dynamics_kernel(int ms, EngineState st, DynOut o) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  EnvS<C>& e = *reinterpret_cast<EnvS<C>*>(smem_raw);
+  const DevModel& m = c_models[ms];
+  const int r = blockIdx.x, lane = threadIdx.x & 31, nv = m.nv;
+  inverse_setup(ms, e, st.pool + (size_t)st.dr_row[r] * m.pool_P, r, (const int*)nullptr);
+  for (int i = lane; i < nv; i += 32) {
+    e.qpos[i] = st.qpos[(size_t)r * nv + i];
+    e.qvel[i] = st.qvel[(size_t)r * nv + i];
+  }
+  __syncwarp();
+  const size_t rv = (size_t)r * nv;
+  DynOut row;
+  row.M = o.M ? o.M + rv * nv : nullptr;
+  row.bias = o.bias ? o.bias + rv : nullptr;
+  row.passive = o.passive ? o.passive + rv : nullptr;
+  row.com = o.com ? o.com + (size_t)r * LS_COM_DIM : nullptr;
+  row.jac = o.jac ? o.jac + rv * m.nb * 6 : nullptr;
+  row.jac_com = o.jac_com ? o.jac_com + rv * 3 : nullptr;
+  dynamics_terms(ms, e, row);
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // Regrouping: the warps of a block run the solver in lock-step, so a block is as slow as its hardest env. Solver effort
 // is strongly correlated from one control step to the next (lag-1 correlation of the per-step Newton iteration count
 // ~0.6), so before every step the envs are bucketed by the iteration count of their previous step (counting sort,
@@ -1141,6 +1169,15 @@ static int launch_dataset_inverse(locosim_handle* h, float* qfrc, cudaStream_t s
   if (rows > 0)
     inverse_kernel<RoundLoop<C>><<<rows, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, h->dt, (const int*)h->d_stage,
                                                                    nullptr, h->d_model_row, dataset_inv_dt(h), qfrc);
+  CK(cudaGetLastError());
+  return 0;
+}
+// dynamics_kernel with inverse_kernel's configuration type: the stages both call (kinematics, com_pos, crb_factor,
+// passive_bias) are then the same functions
+template <class C>
+static int launch_dynamics(locosim_handle* h, const DynOut& o, cudaStream_t s) {
+  static_assert(sizeof(EnvS<C>) <= 48 * 1024, "dynamics_kernel: one EnvS per block within the default shared-memory limit");
+  dynamics_kernel<RoundLoop<C>><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, o);
   CK(cudaGetLastError());
   return 0;
 }
@@ -1336,6 +1373,7 @@ extern "C" int locosim_configs31_dataset_bodies(locosim_handle* h, float* body, 
 extern "C" int locosim_configs31_inverse(locosim_handle* h, const float* qacc, float* qfrc, cudaStream_t s)
     __attribute__((weak));
 extern "C" int locosim_configs31_dataset_inverse(locosim_handle* h, float* qfrc, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_configs31_dynamics(locosim_handle* h, const DynOut* o, cudaStream_t s) __attribute__((weak));
 
 // body_kernel outside a step, for the envs of `mask` (NULL = all), the parts (see body_kernel) that are registered:
 // d_next_body (1) after locosim_reset* and locosim_set_state; the reference keys (2) and d_next_ref (4) after locosim_reset*,
@@ -1577,6 +1615,35 @@ int locosim_create_dataset_inverse(locosim_t* h, float* d_qfrc, void* stream) {
     case 4:
     case 5: return locosim_configs31_dataset_inverse(h, d_qfrc, s);
     default: return launch_dataset_inverse<CfgPyrRK4>(h, d_qfrc, s);
+  }
+}
+int locosim_dynamics_terms(locosim_t* h, float* d_M, float* d_bias, float* d_passive, float* d_com, float* d_jac,
+                           float* d_jac_com, void* stream) {
+  const size_t n = (size_t)h->n_envs, nv = (size_t)h->hm.nv;
+  float* const buf[6] = {d_M, d_bias, d_passive, d_com, d_jac, d_jac_com};
+  const size_t bytes[6] = {n * nv * nv * 4, n * nv * 4, n * nv * 4, n * LS_COM_DIM * 4, n * h->hm.nb * 6 * nv * 4,
+                           n * 3 * nv * 4};
+  bool any = false;
+  for (int i = 0; i < 6; i++) {
+    if (!buf[i]) continue;
+    any = true;
+    for (int j = 0; j < i; j++) {
+      if (!buf[j]) continue;
+      const char *a = (const char*)buf[i], *b = (const char*)buf[j];
+      if (a < b + bytes[j] && b < a + bytes[i]) { h->err = "dynamics_terms outputs overlap"; return 1; }
+    }
+  }
+  if (!any || n == 0) return 0;
+  CK(cudaSetDevice(h->device));
+  const DynOut o = {d_M, d_bias, d_passive, d_com, d_jac, d_jac_com};
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (h->cfg) {
+    case 0: return launch_dynamics<CfgEllEuler>(h, o, s);
+    case 1: return launch_dynamics<CfgPyrEuler>(h, o, s);
+    case 3: return launch_dynamics<CfgPyrEuler29>(h, o, s);
+    case 4:
+    case 5: return locosim_configs31_dynamics(h, &o, s);
+    default: return launch_dynamics<CfgPyrRK4>(h, o, s);
   }
 }
 int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {

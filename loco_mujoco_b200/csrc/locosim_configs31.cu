@@ -95,6 +95,15 @@ int locosim_configs31_inverse(Handle31* h, const float* qacc, float* qfrc, cudaS
   }
 }
 
+int locosim_configs31_dynamics(Handle31* h, const locosim31::DynOut* o, cudaStream_t s) {
+  using namespace locosim31;
+  switch (h->cfg) {
+    case 4: return launch_dynamics<CfgPyrRK4_31>(h, *o, s);
+    case 5: return launch_dynamics<CfgPyrEuler31>(h, *o, s);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
 int locosim_configs31_dataset_inverse(Handle31* h, float* qfrc, cudaStream_t s) {
   using namespace locosim31;
   switch (h->cfg) {

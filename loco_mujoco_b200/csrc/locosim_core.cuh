@@ -2945,6 +2945,100 @@ LS_FN void inverse_dynamics(const int ms, EnvS<C>& e, float* out) {
   SYNC();
 }
 
+// ----------------------------------------------------------------------------------------------------------
+// dynamics terms (locosim_dynamics_terms): M, qfrc_bias, qfrc_passive, the whole-robot CoM and mass, mj_jacBody at xpos of
+// every body and mj_jacSubtreeCom of the robot
+// ----------------------------------------------------------------------------------------------------------
+// one env's rows of the outputs (each may be NULL): M [nv, nv], bias [nv], passive [nv], com [LS_COM_DIM], jac [nb, 6, nv],
+// jac_com [3, nv]
+struct DynOut {
+  float *M, *bias, *passive, *com, *jac, *jac_com;
+};
+
+// The terms for the state e.qpos / e.qvel and the parameters e.prm (the caller has run init_workspace). A non-finite qpos
+// or qvel gives zero rows. Each output is written with nv innermost, one lane per entry.
+//   M:        crb_factor's e.M (dof_armature included).
+//   com:      com_pos's e.com, then the total mass summed as com_pos sums it.
+//   jac:      column d of body b, for d on b's chain: cdof[d] = (w, v) at e.com moved to xpos_b, (w, v + w x (xpos_b - com)),
+//             as body_outputs moves the velocity; 0 elsewhere.
+//   jac_com:  column d = (m_sub v + w x h_sub) / m_total, m_sub and h_sub the mass and first moment about e.com of the
+//             subtree of d's body, which crb_factor's composite inertia crb holds (entries 9 and 6-8).
+//   bias / passive: passive_bias's passes (A) and (B) (RNE at qacc = 0 with gravity; the body forces are left in e.crb), then
+//             its pass (C) here with the two terms kept apart. passive_bias itself is called unchanged, so inverse_kernel
+//             keeps its code; it overwrites crb, so the Jacobians are written first.
+// A whole-warp call; it writes nothing but the outputs and the env's working set.
+template <class C>
+LS_FN void dynamics_terms(const int ms, EnvS<C>& e, const DynOut o) {
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv, nb = m.nb;
+  bool bad = false;
+  PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+#ifndef LS_EMULATE
+  bad = __any_sync(0xffffffffu, bad);
+#endif
+  if (bad) {
+    if (o.M) PAR_FOR(k, nv * nv) o.M[k] = 0.0f;
+    if (o.bias) PAR_FOR(k, nv) o.bias[k] = 0.0f;
+    if (o.passive) PAR_FOR(k, nv) o.passive[k] = 0.0f;
+    if (o.com) PAR_FOR(k, LS_COM_DIM) o.com[k] = 0.0f;
+    if (o.jac) PAR_FOR(k, nb * 6 * nv) o.jac[k] = 0.0f;
+    if (o.jac_com) PAR_FOR(k, 3 * nv) o.jac_com[k] = 0.0f;
+    SYNC();
+    return;
+  }
+  kinematics(ms, e);
+  com_pos(ms, e);
+  if (o.M || o.jac_com) crb_factor(ms, e);
+  float mass = 0;
+  PAR_FOR(b, nb) mass += PRM(body_mass)[b];
+  mass = WARP_SUM(mass);
+  if (o.M) PAR_FOR(k, nv * nv) {
+    const int i = k / nv;
+    o.M[k] = e.M[i][k - i * nv];
+  }
+  if (o.com) PAR_FOR(k, LS_COM_DIM) o.com[k] = k < 3 ? e.com[k] : mass;
+  if (o.jac) PAR_FOR(k, nb * 6 * nv) {
+    const int br = k / nv, d = k - br * nv, b = br / 6, r = br - 6 * b;
+    float x = 0.0f;
+    if (b > 0 && ((m.body_dofmask[b] >> d) & 1)) {
+      const float* cd = e.cdof[d];
+      if (r < 3) {
+        x = cd[r];
+      } else {
+        const int c = r - 3, c1 = c == 2 ? 0 : c + 1, c2 = c == 0 ? 2 : c - 1;
+        const float p1 = e.xpos[b][c1] - e.com[c1], p2 = e.xpos[b][c2] - e.com[c2];
+        x = cd[r] + (cd[c1] * p2 - cd[c2] * p1);
+      }
+    }
+    o.jac[k] = x;
+  }
+  if (o.jac_com) {
+    const float inv = 1.0f / mass;
+    PAR_FOR(k, 3 * nv) {
+      const int c = k / nv, d = k - c * nv, c1 = c == 2 ? 0 : c + 1, c2 = c == 0 ? 2 : c - 1;
+      const float* cd = e.cdof[d];
+      const float* h = e.crb[m.jnt_bodyid[d]];
+      o.jac_com[k] = (h[9] * cd[3 + c] + (cd[c1] * h[6 + c2] - cd[c2] * h[6 + c1])) * inv;
+    }
+  }
+  SYNC();
+  if (o.bias || o.passive) {
+    passive_bias(ms, e);
+    PAR_FOR(j, nv) {
+      float F[6] = {0, 0, 0, 0, 0, 0};
+      NOUNROLL for (int b = 1; b < nb; b++) {
+        if (!((m.body_dofmask[b] >> j) & 1)) continue;
+        for (int c = 0; c < 6; c++) F[c] += e.crb[b][c];
+      }
+      float bias = 0;
+      for (int c = 0; c < 6; c++) bias += e.cdof[j][c] * F[c];
+      if (o.bias) o.bias[j] = bias;
+      if (o.passive) o.passive[j] = -PRM(jnt_stiffness)[j] * (e.qpos[j] - m.qpos_spring[j]) - PRM(dof_damping)[j] * e.qvel[j];
+    }
+    SYNC();
+  }
+}
+
 template <class C>
 LS_FN void euler_step(const int ms, EnvS<C>& e) {
   const DevModel& m = c_models[ms];

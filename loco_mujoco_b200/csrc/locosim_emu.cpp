@@ -32,6 +32,7 @@ struct EmuBase {
   virtual void body(float* out) = 0;
   virtual void ref(const DevTask& t, const float* row, float angle, float* out) = 0;
   virtual void inv(const double* qacc, float* out) = 0;
+  virtual void dyn(const DynOut& o) = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -103,6 +104,11 @@ struct EmuT : EmuBase {
     for (int i = 0; i < m.nv; i++) e.qacc[i] = (float)qacc[i];
     inverse_dynamics(0, e, out);
   }
+  void dyn(const DynOut& o) override {
+    c_models[0] = m;
+    e.substep = -1;
+    dynamics_terms(0, e, o);
+  }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
 
@@ -164,6 +170,12 @@ void emu_reference_row(EmuBase* s, const float* row, const int* recenter, const 
 // with the model's own parameters. Overwrites the env's acceleration and constraint working set (not its state or warm
 // start), as a forward evaluation would.
 void emu_inverse(EmuBase* s, const double* qacc, float* out) { s->inv(qacc, out); }
+// dynamics terms (locosim_dynamics_terms) of the emulated env's current state, with the model's own parameters: row 0 of
+// each output's layout (M fp32 [nv, nv], bias / passive [nv], com [LS_COM_DIM], jac [nb, 6, nv], jac_com [3, nv]; each may
+// be NULL). Overwrites the env's kinematics and smooth-dynamics working set (not its state or warm start).
+void emu_dynamics_terms(EmuBase* s, float* M, float* bias, float* passive, float* com, float* jac, float* jac_com) {
+  s->dyn(DynOut{M, bias, passive, com, jac, jac_com});
+}
 // contact outputs of the emulated env (locosim_set_contact_outputs; row 0 of the engine's layout: fp32 [nb, LS_CONTACT_DIM], or
 // NULL): every later emu_step(ctrl, nsub) runs as one control step of nsub sub-steps and leaves their mean wrench there
 void emu_set_contact(EmuBase* s, float* wrench) { s->cw.wrench = wrench; }

@@ -96,6 +96,8 @@ def load_library():
     lib.locosim_inverse.argtypes = [vp, vp, vp, vp]
     lib.locosim_create_dataset_inverse.restype = ip
     lib.locosim_create_dataset_inverse.argtypes = [vp, vp, vp]
+    lib.locosim_dynamics_terms.restype = ip
+    lib.locosim_dynamics_terms.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -110,7 +112,7 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
                     "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs",
                     "locosim_set_reference_outputs", "locosim_create_dataset_bodies", "locosim_inverse",
-                    "locosim_create_dataset_inverse"]
+                    "locosim_create_dataset_inverse", "locosim_dynamics_terms"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -119,6 +121,8 @@ BODY_DIM = 13
 CONTACT_DIM = 6
 # values per dof row of the dof outputs (include/locosim.h LS_DOF_DIM): qfrc_actuator, qfrc_constraint, qacc
 DOF_DIM = 3
+# values per env of the dynamics terms' centre of mass (include/locosim.h LS_COM_DIM): x, y, z, total mass
+COM_DIM = 4
 
 # bits of the done byte of a step (include/locosim.h)
 DONE_ABSORBING, DONE_TRUNCATED = 1, 2
@@ -448,6 +452,42 @@ class CudaEngine:
         self._check(self.lib.locosim_create_dataset_inverse(self.h, _ptr(out), self._stream()))
         self.launches += 1
         return out
+
+    def dynamics_terms(self, M=None, bias=None, passive=None, com=None, jac=None, jac_com=None):
+        """Dynamics terms of include/locosim.h (locosim_dynamics_terms) of every env at its stored state and parameter-pool
+        row, written into the float32 cuda tensors given (each may be None): M [n_envs, nq, nq] (mj_fullM, armature on the
+        diagonal), bias [n_envs, nq] (qfrc_bias), passive [n_envs, nq] (qfrc_passive), com [n_envs, COM_DIM] (whole-robot
+        CoM x, y, z, then the total mass), jac [n_envs, nbody, 6, nq] (mj_jacBody at each body's xpos: jacr rows, then
+        jacp rows), jac_com [n_envs, 3, nq] (mj_jacSubtreeCom of the robot). The tensors must not overlap. A non-finite
+        state gives that env zero rows. Changes nothing else in the engine; stream-ordered, no allocation (can be captured
+        in a CUDA graph). Returns {name: tensor} of the outputs given; with none given, launches nothing."""
+        t = self.torch
+        n, nq = self.n_envs, self.nq
+        outs = (("M", M, (n, nq, nq)), ("bias", bias, (n, nq)), ("passive", passive, (n, nq)), ("com", com, (n, COM_DIM)),
+                ("jac", jac, (n, self.nbody, 6, nq)), ("jac_com", jac_com, (n, 3, nq)))
+        spans = []
+        for name, x, shape in outs:
+            if x is None:
+                continue
+            if not isinstance(x, t.Tensor) or x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
+                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+            if tuple(x.shape) != shape:
+                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+            size = 4
+            for k in shape:
+                size *= k
+            a = x.data_ptr()
+            for other, b, bsize in spans:
+                if size and bsize and a < b + bsize and b < a + size:
+                    raise ValueError("%s and %s must not overlap" % (name, other))
+            spans.append((name, a, size))
+        given = {name: x for name, x, _ in outs if x is not None}
+        if not given:
+            return given
+        self._check(self.lib.locosim_dynamics_terms(self.h, _ptr(M), _ptr(bias), _ptr(passive), _ptr(com), _ptr(jac),
+                                                     _ptr(jac_com), self._stream()))
+        self.launches += 1
+        return given
 
     def set_goal(self, goal):
         """goal: float32 cuda [n_envs, 4] per-episode goal features (A1: cos, sin, speed)."""

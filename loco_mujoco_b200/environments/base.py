@@ -664,6 +664,48 @@ class LocoEnv:
         return self._get_engine().create_dataset_inverse()
 
     # ---------------------------------------------------------------------------------------------------
+    # dynamics terms (MuJoCo's qM / qfrc_bias / qfrc_passive / subtree_com / mj_jacBody, include/locosim.h
+    # locosim_dynamics_terms)
+    # ---------------------------------------------------------------------------------------------------
+    DYNAMICS_TERMS = ("mass_matrix", "bias", "passive", "com", "body_jacobian", "com_jacobian")
+
+    def dynamics_terms(self, mass_matrix=True, bias=True, passive=True, com=True, body_jacobian=False, com_jacobian=False,
+                       out=None):
+        """The model-based terms of every env at its current state, the state of info["next_obs"], with its parameter-pool
+        row (MuJoCo 2.3.7's meaning), as a dict of float32 torch tensors on the env's device, one key per term asked for:
+            mass_matrix    [num_envs, nq, nq]        M(q) of mj_fullM, dof_armature on the diagonal
+            bias           [num_envs, nq]            qfrc_bias = C(q, qvel) qvel + g(q) (mj_rne at qacc = 0)
+            passive        [num_envs, nq]            qfrc_passive = -stiffness (q - q_spring) - damping qvel
+            com            [num_envs, 4]             the whole-robot centre of mass (x, y, z) and the total mass, a carried
+                                                     weight included (both follow the env's pool row)
+            body_jacobian  [num_envs, nbody, 6, nq]  mj_jacBody at each body's origin xpos (not its CoM), world frame:
+                                                     rows 0-2 angular, rows 3-5 linear, so body_jacobian @ qvel gives
+                                                     body_state[..., 7:13]; body 0 (the world) is zeros
+            com_jacobian   [num_envs, 3, nq]         d(com) / dq (mj_jacSubtreeCom of the robot)
+        so that, away from contacts and joint limits, M qacc + bias - passive = inverse_dynamics(qacc). Dof axes are in the
+        qvel layout (`dof_index(joint)`), body axes in the model's body order (`body_index(name)`). A non-finite state gives
+        that env zero rows. `out`: the dict of an earlier call, filled in place and returned (a graph-captured loop then
+        allocates nothing); terms it lacks are allocated. Changes nothing in the env."""
+        import torch
+        eng = self._get_engine()
+        n, nq = self.num_envs, self._model.nq
+        shapes = dict(mass_matrix=(n, nq, nq), bias=(n, nq), passive=(n, nq), com=(n, 4),
+                      body_jacobian=(n, self._model.nbody, 6, nq), com_jacobian=(n, 3, nq))
+        want = dict(mass_matrix=mass_matrix, bias=bias, passive=passive, com=com, body_jacobian=body_jacobian,
+                    com_jacobian=com_jacobian)
+        if out is None:
+            out = {}
+        elif not isinstance(out, dict):
+            raise ValueError("out must be the dict of an earlier dynamics_terms() call")
+        for k in self.DYNAMICS_TERMS:
+            if want[k] and out.get(k) is None:
+                out[k] = torch.empty(shapes[k], dtype=torch.float32, device=eng.device)
+        got = {k: out[k] if want[k] else None for k in self.DYNAMICS_TERMS}
+        eng.dynamics_terms(M=got["mass_matrix"], bias=got["bias"], passive=got["passive"], com=got["com"],
+                           jac=got["body_jacobian"], jac_com=got["com_jacobian"])
+        return out
+
+    # ---------------------------------------------------------------------------------------------------
     # the hot path
     # ---------------------------------------------------------------------------------------------------
     def reward(self, state, action, next_state, absorbing):

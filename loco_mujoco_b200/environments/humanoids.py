@@ -342,6 +342,13 @@ class HumanoidTorque4AgesAll:
     create_dataset_inverse = _no_inverse_dynamics
     dof_index = _no_inverse_dynamics
 
+    # ---- dynamics terms: likewise ----
+    def _no_dynamics_terms(self, *args, **kwargs):
+        raise NotImplementedError("the dynamics terms (dynamics_terms) are not available for HumanoidTorque4Ages mode 'all': "
+                                  "use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
+
+    dynamics_terms = _no_dynamics_terms
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch
