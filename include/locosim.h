@@ -310,6 +310,41 @@ int locosim_create_dataset_inverse(locosim_t* h, float* d_qfrc, void* stream);
 int locosim_dynamics_terms(locosim_t* h, float* d_M, float* d_bias, float* d_passive, float* d_com, float* d_jac,
                            float* d_jac_com, void* stream);
 
+/* Forward dynamics under a given action, without advancing the env: one MuJoCo 2.3.7 mj_forward per env, followed by
+ * mj_rnePostConstraint. Every env is evaluated
+ *   - at its stored state (what locosim_get_state returns), with its stored qacc_warmstart as the Newton warm start;
+ *   - with its current parameter-pool row (carry tasks: the carried weight's model);
+ *   - with ctrl from d_action [n_envs, action_dim] exactly as locosim_step computes it (action * act_delta + act_mean into
+ *     act_idx; position mode included);
+ *   - with the registered xfrc_applied / qfrc_applied, read as a step reads them;
+ *   - with the solver settings of locosim_set_solver.
+ * The integrator plays no part: for Euler with joint damping, qacc is the explicit mj_forward one, as in the dof outputs.
+ * All outputs are fp32 DEVICE buffers, env-major; dofs in the qvel order, body rows in the compiled model's body indices:
+ *   d_dof       [n_envs, nv, LS_DOF_DIM]          the dof outputs' layout and meaning (qfrc_actuator, qfrc_constraint,
+ *                                                 qacc) for this single evaluation, not a sub-step mean
+ *   d_body_acc  [n_envs, nbody, LS_BODY_ACC_DIM]  per body the angular acceleration (3), then the linear acceleration of the
+ *                                                 body-frame origin xpos MINUS gravity (3), world frame:
+ *                                                 mj_objectAcceleration(m, d, mjOBJ_XBODY, b, res, 0). The angular part is
+ *                                                 d/dt body_state[..., 7:10], the linear part d^2 xpos / dt^2 - gravity, so a
+ *                                                 body resting on the floor reads (0, 0, +9.81) and a free-falling one 0 (an
+ *                                                 accelerometer's reading). Row 0 is (0, 0, 0, -gravity), as d->cacc[0].
+ *   d_cfrc_int  [n_envs, nbody, LS_CONTACT_DIM]   force (3), then torque about xpos (3), world frame: the wrench body b's
+ *                                                 parent exerts on b through the joints between them (d->cfrc_int[b] moved
+ *                                                 from subtree_com to xpos, force first as in the contact outputs). Row 0 is 0.
+ *   d_cfrc_ext  [n_envs, nbody, LS_CONTACT_DIM]   the same layout: the external wrench on b, its contacts (the contact
+ *                                                 outputs' per-contact definition over this evaluation's contact list;
+ *                                                 contacts past the per-env cap are not in it) plus xfrc_applied[b] moved from
+ *                                                 xipos to xpos (d->cfrc_ext). Row 0 is 0.
+ * d_action is required; any output may be NULL, and with all four NULL the call launches nothing and returns 0. Outputs
+ * that overlap each other or d_action are refused. A non-finite qpos, qvel or action of an env gives that env zero rows.
+ * The call changes nothing: state, warm start, counters, cursors, random streams, episode statistics, every registered
+ * output and the dof outputs' actuator scratch stay as they were, so a step after it is bit-identical to the same step
+ * without it. Stream-ordered, no host synchronisation, no allocation: it can be captured in a CUDA graph (a replay reads the
+ * action and the state as they are then). */
+#define LS_BODY_ACC_DIM 6
+int locosim_forward(locosim_t* h, const float* d_action, float* d_dof, float* d_body_acc, float* d_cfrc_int,
+                    float* d_cfrc_ext, void* stream);
+
 /* Per-episode goal features (UnitreeA1: cos / sin of the goal direction and the goal speed, GoalDirectionVelocity set in
  * setup() unitreeA1.py:287-291); normally loaded from the reset table, settable for reset(obs=...) (base.py:217-218,633-654).
  * d_goal fp32 [n_envs, 4]. */

@@ -1042,6 +1042,37 @@ __global__ void __launch_bounds__(32) dynamics_kernel(int ms, EngineState st, Dy
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// Forward dynamics (locosim_forward), inverse_kernel's layout: one warp and one EnvS per block (block = env), at the env's
+// stored state, warm start and parameter-pool row, ctrl from `action` as the step kernels map it, the pair table read as
+// inverse_kernel reads it. EnvS::substep = -1: no output hook of the stages stores anything (smooth_forces leaves the dof
+// outputs' actuator scratch alone). `so` has no block barriers (one warp per block). The engine's state is only read.
+// ----------------------------------------------------------------------------------------------------------
+template <class C>
+__global__ void __launch_bounds__(32) forward_kernel(int ms, EngineState st, DevTask t, const int* __restrict__ pk,
+                                                     SolverOpts so, const float* __restrict__ action, FwdOut o) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  EnvS<C>& e = *reinterpret_cast<EnvS<C>*>(smem_raw);
+  const DevModel& m = c_models[ms];
+  const int r = blockIdx.x, lane = threadIdx.x & 31, nv = m.nv, nu = m.nu, nb = m.nb;
+  inverse_setup(ms, e, st.pool + (size_t)st.dr_row[r] * m.pool_P, r, pk);
+  for (int i = lane; i < nv; i += 32) {
+    e.qpos[i] = st.qpos[(size_t)r * nv + i];
+    e.qvel[i] = st.qvel[(size_t)r * nv + i];
+    e.qacc_ws[i] = st.ws[(size_t)r * nv + i];
+    e.qacc[i] = 0;
+  }
+  for (int i = lane; i < nu; i += 32) e.ctrl[t.act_idx[i]] = action[(size_t)r * nu + i] * t.act_delta[i] + t.act_mean[i];
+  if (lane == 0) e.iter_sum = 0;
+  __syncwarp();
+  FwdOut row;
+  row.dof = o.dof ? o.dof + (size_t)r * nv * LS_DOF_DIM : nullptr;
+  row.body_acc = o.body_acc ? o.body_acc + (size_t)r * nb * LS_BODY_ACC_DIM : nullptr;
+  row.cfrc_int = o.cfrc_int ? o.cfrc_int + (size_t)r * nb * LS_CONTACT_DIM : nullptr;
+  row.cfrc_ext = o.cfrc_ext ? o.cfrc_ext + (size_t)r * nb * LS_CONTACT_DIM : nullptr;
+  forward_dynamics(ms, e, so, row);
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // Regrouping: the warps of a block run the solver in lock-step, so a block is as slow as its hardest env. Solver effort
 // is strongly correlated from one control step to the next (lag-1 correlation of the per-step Newton iteration count
 // ~0.6), so before every step the envs are bucketed by the iteration count of their previous step (counting sort,
@@ -1178,6 +1209,19 @@ template <class C>
 static int launch_dynamics(locosim_handle* h, const DynOut& o, cudaStream_t s) {
   static_assert(sizeof(EnvS<C>) <= 48 * 1024, "dynamics_kernel: one EnvS per block within the default shared-memory limit");
   dynamics_kernel<RoundLoop<C>><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, o);
+  CK(cudaGetLastError());
+  return 0;
+}
+// forward_kernel with inverse_kernel's configuration type and pair table (the same contact list as the step kernels' first
+// evaluation of a control step) and the handle's solver settings without block barriers
+template <class C>
+static int launch_forward(locosim_handle* h, const float* action, const FwdOut& o, cudaStream_t s) {
+  static_assert(sizeof(EnvS<C>) <= 48 * 1024, "forward_kernel: one EnvS per block within the default shared-memory limit");
+  SolverOpts so = h->so;
+  so.sync_iters = 0;
+  so.sync_phases = 0;
+  forward_kernel<RoundLoop<C>><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, h->dt, (const int*)h->d_stage, so,
+                                                                       action, o);
   CK(cudaGetLastError());
   return 0;
 }
@@ -1374,6 +1418,8 @@ extern "C" int locosim_configs31_inverse(locosim_handle* h, const float* qacc, f
     __attribute__((weak));
 extern "C" int locosim_configs31_dataset_inverse(locosim_handle* h, float* qfrc, cudaStream_t s) __attribute__((weak));
 extern "C" int locosim_configs31_dynamics(locosim_handle* h, const DynOut* o, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_configs31_forward(locosim_handle* h, const float* action, const FwdOut* o, cudaStream_t s)
+    __attribute__((weak));
 
 // body_kernel outside a step, for the envs of `mask` (NULL = all), the parts (see body_kernel) that are registered:
 // d_next_body (1) after locosim_reset* and locosim_set_state; the reference keys (2) and d_next_ref (4) after locosim_reset*,
@@ -1644,6 +1690,37 @@ int locosim_dynamics_terms(locosim_t* h, float* d_M, float* d_bias, float* d_pas
     case 4:
     case 5: return locosim_configs31_dynamics(h, &o, s);
     default: return launch_dynamics<CfgPyrRK4>(h, o, s);
+  }
+}
+int locosim_forward(locosim_t* h, const float* d_action, float* d_dof, float* d_body_acc, float* d_cfrc_int,
+                    float* d_cfrc_ext, void* stream) {
+  if (!d_action) { h->err = "null action buffer"; return 1; }
+  const size_t n = (size_t)h->n_envs, nv = (size_t)h->hm.nv, nb = (size_t)h->hm.nb;
+  // the action is buffer 0: every output is checked against it and against the outputs before it
+  const char* const buf[5] = {(const char*)d_action, (const char*)d_dof, (const char*)d_body_acc, (const char*)d_cfrc_int,
+                              (const char*)d_cfrc_ext};
+  const size_t bytes[5] = {n * h->hm.nu * 4, n * nv * LS_DOF_DIM * 4, n * nb * LS_BODY_ACC_DIM * 4,
+                           n * nb * LS_CONTACT_DIM * 4, n * nb * LS_CONTACT_DIM * 4};
+  bool any = false;
+  for (int i = 1; i < 5; i++) {
+    if (!buf[i]) continue;
+    any = true;
+    for (int j = 0; j < i; j++) {
+      if (!buf[j]) continue;
+      if (buf[i] < buf[j] + bytes[j] && buf[j] < buf[i] + bytes[i]) { h->err = "forward outputs overlap"; return 1; }
+    }
+  }
+  if (!any || n == 0) return 0;
+  CK(cudaSetDevice(h->device));
+  const FwdOut o = {d_dof, d_body_acc, d_cfrc_int, d_cfrc_ext};
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (h->cfg) {
+    case 0: return launch_forward<CfgEllEuler>(h, d_action, o, s);
+    case 1: return launch_forward<CfgPyrEuler>(h, d_action, o, s);
+    case 3: return launch_forward<CfgPyrEuler29>(h, d_action, o, s);
+    case 4:
+    case 5: return locosim_configs31_forward(h, d_action, &o, s);
+    default: return launch_forward<CfgPyrRK4>(h, d_action, o, s);
   }
 }
 int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {

@@ -104,6 +104,15 @@ int locosim_configs31_dynamics(Handle31* h, const locosim31::DynOut* o, cudaStre
   }
 }
 
+int locosim_configs31_forward(Handle31* h, const float* action, const locosim31::FwdOut* o, cudaStream_t s) {
+  using namespace locosim31;
+  switch (h->cfg) {
+    case 4: return launch_forward<CfgPyrRK4_31>(h, action, *o, s);
+    case 5: return launch_forward<CfgPyrEuler31>(h, action, *o, s);
+    default: h->err = "not a 31-dof configuration"; return 1;
+  }
+}
+
 int locosim_configs31_dataset_inverse(Handle31* h, float* qfrc, cudaStream_t s) {
   using namespace locosim31;
   switch (h->cfg) {

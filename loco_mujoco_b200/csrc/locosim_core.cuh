@@ -3266,6 +3266,192 @@ LS_FN void physics_substeps(const int ms, EnvS<C>& e, const SolverOpts so, int n
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// forward dynamics outputs (locosim_forward): one mj_forward, then mj_rnePostConstraint's body accelerations and forces
+// ----------------------------------------------------------------------------------------------------------
+// one env's rows of the outputs (each may be NULL): dof [nv, LS_DOF_DIM], body_acc [nb, LS_BODY_ACC_DIM], cfrc_int and
+// cfrc_ext [nb, LS_CONTACT_DIM]
+struct FwdOut {
+  float *dof, *body_acc, *cfrc_int, *cfrc_ext;
+};
+
+// the force of actuator i at the env's state and e.ctrl: smooth_forces' expression (before the gear), which stores the
+// force only while the dof outputs are registered and only inside a step
+template <class C>
+LS_DEV float actuator_force(const DevModel& m, const EnvS<C>& e, const int i) {
+  float c = e.ctrl[i];
+  if (m.actuator_ctrllimited[i]) c = fminf(m.actuator_ctrlrange[2 * i + 1], fmaxf(m.actuator_ctrlrange[2 * i], c));
+  const int d = m.actuator_dof[i];
+  float f = m.actuator_gain[i] * c + m.actuator_bias[3 * i] + m.actuator_bias[3 * i + 1] * e.qpos[d] +
+            m.actuator_bias[3 * i + 2] * e.qvel[d];
+  if (m.actuator_forcelimited[i]) f = fminf(m.actuator_forcerange[2 * i + 1], fmaxf(m.actuator_forcerange[2 * i], f));
+  return f;
+}
+
+// The outputs of the forward evaluation forward() has just made (the caller ran it at e.qpos / e.qvel / e.ctrl). In order:
+//   (1) the dof row: per dof the sum of gear * actuator_force over its actuators in actuator order, qfrc_constraint and
+//       qacc, read before anything below overwrites the storage they share with cinert / cdof_dot;
+//   (2) cfrc_ext from the contacts, one lane per body, as contact_wrench sums them (force, torque about xpos, world);
+//   (3) kinematics and com_pos again (xipos, ximat, cinert and the joint frames lie under the constraint rows; both are
+//       deterministic functions of qpos, so xpos, com and cdof come out with the same bits), cdof_dot as passive_bias
+//       builds it, and the applied wrench xfrc_applied[b], moved from xipos to xpos, added to cfrc_ext;
+//   (4) per body cvel and cacc = -g + sum over its chain of (cdof qacc + cdof_dot qvel) (spatial, about com); body_acc is
+//       mj_objectAcceleration at xpos: (alpha, a + alpha x r + w x (v + w x r)), r = xpos - com; the body force
+//       f = cinert cacc + cvel x* (cinert cvel) - cfrc_ext (about com);
+//   (5) cfrc_int[b] = the sum of f over b's subtree (b and its descendants, in body order), moved to xpos.
+// cfrc_ext and f are kept in e.H (the Newton Hessian's factor, dead after the solve). Row 0 of body_acc is (0, -g), of
+// cfrc_int and cfrc_ext zeros. A whole-warp call; it writes nothing but the outputs and the env's working set.
+template <class C>
+LS_FN void forward_outputs(const int ms, EnvS<C>& e, const FwdOut o) {
+  typedef EnvS<C> E;
+  static_assert(C::NB <= 32, "forward_outputs: one lane per body");
+  static_assert(2 * E::NB * 6 <= E::NV * E::NVP, "forward_outputs: cfrc_ext and the body forces fit in H");
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv, nb = m.nb, nu = m.nu;
+  if (o.dof) PAR_FOR(j, nv) {
+    float fa = 0;
+    NOUNROLL for (int i = 0; i < nu; i++) if (m.actuator_dof[i] == j) fa += m.actuator_gear[i] * actuator_force(m, e, i);
+    float* dst = o.dof + j * LS_DOF_DIM;
+    dst[0] = fa; dst[1] = e.qfrc_constraint[j]; dst[2] = e.qacc[j];
+  }
+  SYNC();
+  if (!o.body_acc && !o.cfrc_int && !o.cfrc_ext) return;
+  float (*ext)[6] = reinterpret_cast<float (*)[6]>(&e.H[0][0]);
+  float (*frc)[6] = ext + E::NB;
+  const bool need_ext = o.cfrc_ext || o.cfrc_int;
+  if (need_ext) {
+    const int ncon = e.ncon;
+    PAR_FOR(b, nb) {
+      float w[6] = {0, 0, 0, 0, 0, 0};
+      if (b > 0) {
+        NOUNROLL for (int ci = 0; ci < ncon; ci++) {
+          const int b1 = m.geom_bodyid[e.con_g1[ci]], b2 = m.geom_bodyid[e.con_g2[ci]];
+          if (b != b1 && b != b2) continue;
+          float f[6];
+          contact_frame_force(e, ci, f);
+          const float* fr = e.con_frame[ci];
+          float F[3], T[3], rxF[3];
+          for (int c = 0; c < 3; c++) {
+            F[c] = f[0] * fr[c] + f[1] * fr[3 + c] + f[2] * fr[6 + c];
+            T[c] = f[3] * fr[c] + f[4] * fr[3 + c] + f[5] * fr[6 + c];
+          }
+          const float r[3] = {e.con_pos[ci][0] - e.xpos[b][0], e.con_pos[ci][1] - e.xpos[b][1], e.con_pos[ci][2] - e.xpos[b][2]};
+          cross3(rxF, r, F);
+          const float s = b == b2 ? 1.0f : -1.0f;    // (the frame normal points from geom1 to geom2)
+          for (int c = 0; c < 3; c++) { w[c] += s * F[c]; w[3 + c] += s * (rxF[c] + T[c]); }
+        }
+      }
+      for (int c = 0; c < 6; c++) ext[b][c] = w[c];
+    }
+    SYNC();
+  }
+  kinematics(ms, e);
+  com_pos(ms, e);
+  PAR_FOR(j, nv) {
+    unsigned mask = (unsigned)m.body_dofmask[m.jnt_bodyid[j]] & ((1u << j) - 1u);
+    float v[6] = {0, 0, 0, 0, 0, 0};
+    while (mask) {
+      const int i = LS_FFS(mask) - 1;
+      mask &= mask - 1;
+      const float qv = e.qvel[i];
+      for (int c = 0; c < 6; c++) v[c] = fmaf(e.cdof[i][c], qv, v[c]);
+    }
+    float cdd[6];
+    crossMotion(cdd, v, e.cdof[j]);
+    for (int c = 0; c < 6; c++) e.cdof_dot[j][c] = cdd[c];
+  }
+  const float* __restrict__ xfrc = c_applied[ms].xfrc;
+  if (need_ext && xfrc) PAR_FOR(b, nb) {
+    if (b == 0) continue;
+    const float* w = xfrc + ((size_t)e.env * nb + b) * 6;
+    const float F[3] = {LS_LDG(w), LS_LDG(w + 1), LS_LDG(w + 2)};
+    const float r[3] = {e.xipos[b][0] - e.xpos[b][0], e.xipos[b][1] - e.xpos[b][1], e.xipos[b][2] - e.xpos[b][2]};
+    float rxF[3];
+    cross3(rxF, r, F);
+    for (int c = 0; c < 3; c++) { ext[b][c] += F[c]; ext[b][3 + c] += rxF[c] + LS_LDG(w + 3 + c); }
+  }
+  SYNC();
+  if (o.cfrc_ext) PAR_FOR(k, nb * LS_CONTACT_DIM) o.cfrc_ext[k] = ext[k / 6][k % 6];
+  PAR_FOR(b, nb) {
+    unsigned mask = b > 0 ? (unsigned)m.body_dofmask[b] : 0u;
+    float cvel[6] = {0, 0, 0, 0, 0, 0}, cacc[6] = {0, 0, 0, -m.gravity[0], -m.gravity[1], -m.gravity[2]};
+    while (mask) {
+      const int i = LS_FFS(mask) - 1;
+      mask &= mask - 1;
+      const float qv = e.qvel[i], qa = e.qacc[i];
+      for (int c = 0; c < 6; c++) {
+        cvel[c] = fmaf(e.cdof[i][c], qv, cvel[c]);
+        cacc[c] = fmaf(e.cdof_dot[i][c], qv, fmaf(e.cdof[i][c], qa, cacc[c]));
+      }
+    }
+    const float r[3] = {e.xpos[b][0] - e.com[0], e.xpos[b][1] - e.com[1], e.xpos[b][2] - e.com[2]};
+    if (o.body_acc) {
+      float wr[3], ar[3], vp[3], wv[3];
+      cross3(wr, cvel, r);
+      cross3(ar, cacc, r);
+      for (int c = 0; c < 3; c++) vp[c] = cvel[3 + c] + wr[c];
+      cross3(wv, cvel, vp);
+      float* dst = o.body_acc + b * LS_BODY_ACC_DIM;
+      for (int c = 0; c < 3; c++) { dst[c] = cacc[c]; dst[3 + c] = cacc[3 + c] + ar[c] + wv[c]; }
+    }
+    if (o.cfrc_int) {
+      float* f = frc[b];
+      if (b == 0) { for (int c = 0; c < 6; c++) f[c] = 0; continue; }
+      float t1[6], t2[6], t3[6], rxF[3];
+      mulInertVec(t1, e.cinert[b], cacc);
+      mulInertVec(t2, e.cinert[b], cvel);
+      crossForce(t3, cvel, t2);
+      // cfrc_ext about com: torque + (xpos - com) x force
+      cross3(rxF, r, ext[b]);
+      for (int c = 0; c < 3; c++) { f[c] = t1[c] + t3[c] - (ext[b][3 + c] + rxF[c]); f[3 + c] = t1[3 + c] + t3[3 + c] - ext[b][c]; }
+    }
+  }
+  SYNC();
+  if (o.cfrc_int) PAR_FOR(b, nb) {
+    float F[6] = {0, 0, 0, 0, 0, 0};
+    if (b > 0) {
+      for (int c = 0; c < 6; c++) F[c] = frc[b][c];
+      NOUNROLL for (int k = b + 1; k < nb; k++) {
+        int a = m.body_parentid[k];
+        while (a > b) a = m.body_parentid[a];
+        if (a != b) continue;
+        for (int c = 0; c < 6; c++) F[c] += frc[k][c];
+      }
+    }
+    // about xpos: torque + (com - xpos) x force
+    const float r[3] = {e.com[0] - e.xpos[b][0], e.com[1] - e.xpos[b][1], e.com[2] - e.xpos[b][2]};
+    float rxF[3];
+    cross3(rxF, r, F + 3);
+    float* dst = o.cfrc_int + b * LS_CONTACT_DIM;
+    for (int c = 0; c < 3; c++) { dst[c] = b > 0 ? F[3 + c] : 0.0f; dst[3 + c] = b > 0 ? F[c] + rxF[c] : 0.0f; }
+  }
+  SYNC();
+}
+
+// locosim_forward's evaluation of one env: forward() at e.qpos / e.qvel / e.ctrl (the caller ran init_workspace and loaded
+// the warm start), then forward_outputs. A non-finite qpos, qvel or ctrl gives zero rows before anything is evaluated.
+template <class C>
+LS_FN void forward_dynamics(const int ms, EnvS<C>& e, const SolverOpts so, const FwdOut o) {
+  const DevModel& m = c_models[ms];
+  const int nv = m.nv, nb = m.nb, nu = m.nu;
+  bool bad = false;
+  PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+  PAR_FOR(i, nu) bad |= !isfinite(e.ctrl[i]);
+#ifndef LS_EMULATE
+  bad = __any_sync(0xffffffffu, bad);
+#endif
+  if (bad) {
+    if (o.dof) PAR_FOR(k, nv * LS_DOF_DIM) o.dof[k] = 0.0f;
+    if (o.body_acc) PAR_FOR(k, nb * LS_BODY_ACC_DIM) o.body_acc[k] = 0.0f;
+    if (o.cfrc_int) PAR_FOR(k, nb * LS_CONTACT_DIM) o.cfrc_int[k] = 0.0f;
+    if (o.cfrc_ext) PAR_FOR(k, nb * LS_CONTACT_DIM) o.cfrc_ext[k] = 0.0f;
+    SYNC();
+    return;
+  }
+  forward(ms, e, so);
+  forward_outputs(ms, e, o);
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // task layer: observation gather, termination, reward, reset from the trajectory table
 // ----------------------------------------------------------------------------------------------------------
 template <class C>

@@ -33,6 +33,7 @@ struct EmuBase {
   virtual void ref(const DevTask& t, const float* row, float angle, float* out) = 0;
   virtual void inv(const double* qacc, float* out) = 0;
   virtual void dyn(const DynOut& o) = 0;
+  virtual void fwd_out(const double* ctrl, const FwdOut& o) = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -109,6 +110,13 @@ struct EmuT : EmuBase {
     e.substep = -1;
     dynamics_terms(0, e, o);
   }
+  void fwd_out(const double* ctrl, const FwdOut& o) override {
+    for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
+    c_models[0] = m; c_applied[0] = ap;
+    e.substep = -1;
+    init_workspace(0, e);
+    forward_dynamics(0, e, so, o);
+  }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
 
@@ -175,6 +183,13 @@ void emu_inverse(EmuBase* s, const double* qacc, float* out) { s->inv(qacc, out)
 // be NULL). Overwrites the env's kinematics and smooth-dynamics working set (not its state or warm start).
 void emu_dynamics_terms(EmuBase* s, float* M, float* bias, float* passive, float* com, float* jac, float* jac_com) {
   s->dyn(DynOut{M, bias, passive, com, jac, jac_com});
+}
+// forward dynamics (locosim_forward) of the emulated env's current state and warm start at ctrl [nu] (fp64; the engine's
+// ctrl, not the action), with the applied forces of emu_set_applied and the model's own parameters: row 0 of each output's
+// layout (dof fp32 [nv, LS_DOF_DIM], body_acc [nb, LS_BODY_ACC_DIM], cfrc_int / cfrc_ext [nb, LS_CONTACT_DIM]; each may be
+// NULL). Leaves the state as it was; the warm start becomes this evaluation's qacc, as after emu_forward.
+void emu_forward_outputs(EmuBase* s, const double* ctrl, float* dof, float* body_acc, float* cfrc_int, float* cfrc_ext) {
+  s->fwd_out(ctrl, FwdOut{dof, body_acc, cfrc_int, cfrc_ext});
 }
 // contact outputs of the emulated env (locosim_set_contact_outputs; row 0 of the engine's layout: fp32 [nb, LS_CONTACT_DIM], or
 // NULL): every later emu_step(ctrl, nsub) runs as one control step of nsub sub-steps and leaves their mean wrench there

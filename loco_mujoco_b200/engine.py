@@ -98,6 +98,8 @@ def load_library():
     lib.locosim_create_dataset_inverse.argtypes = [vp, vp, vp]
     lib.locosim_dynamics_terms.restype = ip
     lib.locosim_dynamics_terms.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.locosim_forward.restype = ip
+    lib.locosim_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -112,7 +114,7 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
                     "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs",
                     "locosim_set_reference_outputs", "locosim_create_dataset_bodies", "locosim_inverse",
-                    "locosim_create_dataset_inverse", "locosim_dynamics_terms"]
+                    "locosim_create_dataset_inverse", "locosim_dynamics_terms", "locosim_forward"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -123,6 +125,9 @@ CONTACT_DIM = 6
 DOF_DIM = 3
 # values per env of the dynamics terms' centre of mass (include/locosim.h LS_COM_DIM): x, y, z, total mass
 COM_DIM = 4
+# values per body row of the forward dynamics' body accelerations (include/locosim.h LS_BODY_ACC_DIM): angular acceleration
+# (3), linear acceleration of the body-frame origin minus gravity (3), world frame
+BODY_ACC_DIM = 6
 
 # bits of the done byte of a step (include/locosim.h)
 DONE_ABSORBING, DONE_TRUNCATED = 1, 2
@@ -486,6 +491,47 @@ class CudaEngine:
             return given
         self._check(self.lib.locosim_dynamics_terms(self.h, _ptr(M), _ptr(bias), _ptr(passive), _ptr(com), _ptr(jac),
                                                      _ptr(jac_com), self._stream()))
+        self.launches += 1
+        return given
+
+    def forward(self, action, dof=None, body_acc=None, cfrc_int=None, cfrc_ext=None):
+        """Forward dynamics of include/locosim.h (locosim_forward: one mj_forward, then mj_rnePostConstraint) of every env at
+        its stored state, warm start and parameter-pool row under `action` float32 cuda [n_envs, action_dim] (mapped to
+        ctrl as a step maps it), with the registered applied forces; written into the float32 cuda tensors given (each may
+        be None): dof [n_envs, nq, DOF_DIM] (qfrc_actuator, qfrc_constraint, qacc of this evaluation), body_acc
+        [n_envs, nbody, BODY_ACC_DIM] (angular acceleration, linear acceleration of xpos minus gravity), cfrc_int and
+        cfrc_ext [n_envs, nbody, CONTACT_DIM] (force, torque about xpos: from the parent through the joints, and external).
+        The tensors must not overlap each other or `action`. A non-finite state or action gives that env zero rows. Changes
+        nothing in the engine; stream-ordered, no allocation (can be captured in a CUDA graph). Returns {name: tensor} of the
+        outputs given; with none given, launches nothing."""
+        if action is None:
+            raise ValueError("action is required")
+        t = self.torch
+        n, nq, nb = self.n_envs, self.nq, self.nbody
+        outs = (("action", action, (n, self.action_dim)), ("dof", dof, (n, nq, DOF_DIM)),
+                ("body_acc", body_acc, (n, nb, BODY_ACC_DIM)), ("cfrc_int", cfrc_int, (n, nb, CONTACT_DIM)),
+                ("cfrc_ext", cfrc_ext, (n, nb, CONTACT_DIM)))
+        spans = []
+        for name, x, shape in outs:
+            if x is None:
+                continue
+            if not isinstance(x, t.Tensor) or x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
+                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+            if tuple(x.shape) != shape:
+                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+            size = 4
+            for k in shape:
+                size *= k
+            a = x.data_ptr()
+            for other, b, bsize in spans:
+                if size and bsize and a < b + bsize and b < a + size:
+                    raise ValueError("%s and %s must not overlap" % (name, other))
+            spans.append((name, a, size))
+        given = {name: x for name, x, _ in outs[1:] if x is not None}
+        if not given:
+            return given
+        self._check(self.lib.locosim_forward(self.h, _ptr(action), _ptr(dof), _ptr(body_acc), _ptr(cfrc_int), _ptr(cfrc_ext),
+                                             self._stream()))
         self.launches += 1
         return given
 

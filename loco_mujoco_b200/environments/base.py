@@ -706,6 +706,47 @@ class LocoEnv:
         return out
 
     # ---------------------------------------------------------------------------------------------------
+    # forward dynamics under an action (MuJoCo's mj_forward + mj_rnePostConstraint: qacc, cacc, cfrc_int, cfrc_ext,
+    # include/locosim.h locosim_forward)
+    # ---------------------------------------------------------------------------------------------------
+    FORWARD_OUTPUTS = ("dof", "body_acc", "cfrc_int", "cfrc_ext")
+
+    def forward_dynamics(self, action, dof=True, body_acc=True, cfrc_int=False, cfrc_ext=False, out=None):
+        """What `action` would do at every env's current state, the state of info["next_obs"], without advancing it: one
+        MuJoCo 2.3.7 mj_forward with ctrl mapped from `action` (float32 [num_envs, action_dim] on the env's device) as step()
+        maps it, the env's warm start, parameter-pool row and registered xfrc_applied / qfrc_applied, followed by
+        mj_rnePostConstraint. Returns a dict of float32 torch tensors on the env's device, one key per output asked for:
+            dof       [num_envs, nq, 3]     qfrc_actuator, qfrc_constraint, qacc of this evaluation (dof_outputs' layout;
+                                            for Euler, qacc is the explicit mj_forward one, as there)
+            body_acc  [num_envs, nbody, 6]  per body the angular acceleration, then the linear acceleration of its origin
+                                            xpos minus gravity, world frame (mj_objectAcceleration; an accelerometer at
+                                            xpos reads the linear part rotated into its frame: (0, 0, +9.81) at rest)
+            cfrc_int  [num_envs, nbody, 6]  the wrench the parent exerts on the body through the joints between them:
+                                            force, then torque about xpos, world frame (MuJoCo's cfrc_int; a force /
+                                            torque sensor at the body's joint). Row 0 is zeros
+            cfrc_ext  [num_envs, nbody, 6]  the external wrench on the body, contacts plus xfrc_applied, in the same layout
+                                            (MuJoCo's cfrc_ext). Row 0 is zeros
+        Dof axes are in the qvel layout (`dof_index(joint)`), body axes in the model's body order (`body_index(name)`). A
+        non-finite state or action gives that env zero rows. `out`: the dict of an earlier call, filled in place and
+        returned (a graph-captured loop then allocates nothing); outputs it lacks are allocated. Changes nothing in the env:
+        the next step() is the same, bit for bit, as without this call."""
+        import torch
+        eng = self._get_engine()
+        n, nq, nb = self.num_envs, self._model.nq, self._model.nbody
+        shapes = dict(dof=(n, nq, 3), body_acc=(n, nb, 6), cfrc_int=(n, nb, 6), cfrc_ext=(n, nb, 6))
+        want = dict(dof=dof, body_acc=body_acc, cfrc_int=cfrc_int, cfrc_ext=cfrc_ext)
+        if out is None:
+            out = {}
+        elif not isinstance(out, dict):
+            raise ValueError("out must be the dict of an earlier forward_dynamics() call")
+        for k in self.FORWARD_OUTPUTS:
+            if want[k] and out.get(k) is None:
+                out[k] = torch.empty(shapes[k], dtype=torch.float32, device=eng.device)
+        got = {k: out[k] if want[k] else None for k in self.FORWARD_OUTPUTS}
+        eng.forward(action, **got)
+        return out
+
+    # ---------------------------------------------------------------------------------------------------
     # the hot path
     # ---------------------------------------------------------------------------------------------------
     def reward(self, state, action, next_state, absorbing):

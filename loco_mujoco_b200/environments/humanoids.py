@@ -349,6 +349,13 @@ class HumanoidTorque4AgesAll:
 
     dynamics_terms = _no_dynamics_terms
 
+    # ---- forward dynamics: likewise ----
+    def _no_forward_dynamics(self, *args, **kwargs):
+        raise NotImplementedError("the forward dynamics (forward_dynamics) are not available for HumanoidTorque4Ages mode "
+                                  "'all': use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
+
+    forward_dynamics = _no_forward_dynamics
+
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
         import torch

@@ -19,8 +19,9 @@ def shard_range(n_total, world_size, rank):
 def make_sharded(task_id, n_total, rank=None, world_size=None, device=None, seed=0, **kwargs):
     """LocoEnv for this rank's shard; `env_id_offset` keeps every env's random stream identical to the 1-GPU run.
     Its `xfrc_applied` / `qfrc_applied`, `body_state` / `next_body_state`, `reference_body_state` /
-    `next_reference_body_state`, `contact_wrench` and `dof_outputs`, and what `inverse_dynamics(qacc)` takes and returns
-    and `dynamics_terms()` returns, hold the rows of this shard's envs only (global env offset + i is row i)."""
+    `next_reference_body_state`, `contact_wrench` and `dof_outputs`, what `inverse_dynamics(qacc)` and
+    `forward_dynamics(action)` take and return and what `dynamics_terms()` returns hold the rows of this shard's envs only
+    (global env offset + i is row i)."""
     from . import LocoEnv
     rank = dist.get_rank() if rank is None else rank
     world_size = dist.get_world_size() if world_size is None else world_size
@@ -141,8 +142,8 @@ class MixedBatch:
     Applied forces are per member: `envs[i].xfrc_applied` / `envs[i].qfrc_applied` / `envs[i].body_index(name)`.
     So are body outputs: `envs[i].body_state` / `envs[i].next_body_state`, reference outputs:
     `envs[i].reference_body_state` / `envs[i].next_reference_body_state`, contact outputs: `envs[i].contact_wrench`, dof
-    outputs: `envs[i].dof_outputs`, inverse dynamics: `envs[i].inverse_dynamics(qacc)` / `envs[i].dof_index(joint)`, and
-    dynamics terms: `envs[i].dynamics_terms(...)`.
+    outputs: `envs[i].dof_outputs`, inverse dynamics: `envs[i].inverse_dynamics(qacc)` / `envs[i].dof_index(joint)`,
+    dynamics terms: `envs[i].dynamics_terms(...)`, and forward dynamics: `envs[i].forward_dynamics(action, ...)`.
     """
 
     def __init__(self, members, device="cuda:0", seed=0, env_id_offset=0, concurrent=True, balance=True, stagger_us=40.0, **common):
