@@ -1633,11 +1633,24 @@ int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_bod
     default: return launch_dataset_bodies<CfgPyrRK4>(h, d_body, d_next_body, s);
   }
 }
+// whether any two of the caller's `n` buffers (NULL: skipped) share a byte; bytes[i] is buffer i's size
+static bool buffers_overlap(const void* const* buf, const size_t* bytes, int n) {
+  for (int i = 0; i < n; i++) {
+    if (!buf[i]) continue;
+    for (int j = 0; j < i; j++) {
+      if (!buf[j]) continue;
+      const char *a = (const char*)buf[i], *b = (const char*)buf[j];
+      if (a < b + bytes[j] && b < a + bytes[i]) return true;
+    }
+  }
+  return false;
+}
 int locosim_inverse(locosim_t* h, const float* d_qacc, float* d_qfrc_inverse, void* stream) {
   if (!d_qacc || !d_qfrc_inverse) { h->err = "null buffer"; return 1; }
   const size_t bytes = (size_t)h->n_envs * h->hm.nv * 4;
-  const char *a = (const char*)d_qacc, *b = (const char*)d_qfrc_inverse;
-  if (a < b + bytes && b < a + bytes) { h->err = "qacc and qfrc_inverse overlap"; return 1; }
+  const void* const buf[2] = {d_qacc, d_qfrc_inverse};
+  const size_t sizes[2] = {bytes, bytes};
+  if (buffers_overlap(buf, sizes, 2)) { h->err = "qacc and qfrc_inverse overlap"; return 1; }
   CK(cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)stream;
   switch (h->cfg) {
@@ -1666,20 +1679,11 @@ int locosim_create_dataset_inverse(locosim_t* h, float* d_qfrc, void* stream) {
 int locosim_dynamics_terms(locosim_t* h, float* d_M, float* d_bias, float* d_passive, float* d_com, float* d_jac,
                            float* d_jac_com, void* stream) {
   const size_t n = (size_t)h->n_envs, nv = (size_t)h->hm.nv;
-  float* const buf[6] = {d_M, d_bias, d_passive, d_com, d_jac, d_jac_com};
+  const void* const buf[6] = {d_M, d_bias, d_passive, d_com, d_jac, d_jac_com};
   const size_t bytes[6] = {n * nv * nv * 4, n * nv * 4, n * nv * 4, n * LS_COM_DIM * 4, n * h->hm.nb * 6 * nv * 4,
                            n * 3 * nv * 4};
-  bool any = false;
-  for (int i = 0; i < 6; i++) {
-    if (!buf[i]) continue;
-    any = true;
-    for (int j = 0; j < i; j++) {
-      if (!buf[j]) continue;
-      const char *a = (const char*)buf[i], *b = (const char*)buf[j];
-      if (a < b + bytes[j] && b < a + bytes[i]) { h->err = "dynamics_terms outputs overlap"; return 1; }
-    }
-  }
-  if (!any || n == 0) return 0;
+  if (buffers_overlap(buf, bytes, 6)) { h->err = "dynamics_terms outputs overlap"; return 1; }
+  if (!(d_M || d_bias || d_passive || d_com || d_jac || d_jac_com) || n == 0) return 0;
   CK(cudaSetDevice(h->device));
   const DynOut o = {d_M, d_bias, d_passive, d_com, d_jac, d_jac_com};
   cudaStream_t s = (cudaStream_t)stream;
@@ -1696,21 +1700,12 @@ int locosim_forward(locosim_t* h, const float* d_action, float* d_dof, float* d_
                     float* d_cfrc_ext, void* stream) {
   if (!d_action) { h->err = "null action buffer"; return 1; }
   const size_t n = (size_t)h->n_envs, nv = (size_t)h->hm.nv, nb = (size_t)h->hm.nb;
-  // the action is buffer 0: every output is checked against it and against the outputs before it
-  const char* const buf[5] = {(const char*)d_action, (const char*)d_dof, (const char*)d_body_acc, (const char*)d_cfrc_int,
-                              (const char*)d_cfrc_ext};
+  // the action is buffer 0: every output is checked against it and against the other outputs
+  const void* const buf[5] = {d_action, d_dof, d_body_acc, d_cfrc_int, d_cfrc_ext};
   const size_t bytes[5] = {n * h->hm.nu * 4, n * nv * LS_DOF_DIM * 4, n * nb * LS_BODY_ACC_DIM * 4,
                            n * nb * LS_CONTACT_DIM * 4, n * nb * LS_CONTACT_DIM * 4};
-  bool any = false;
-  for (int i = 1; i < 5; i++) {
-    if (!buf[i]) continue;
-    any = true;
-    for (int j = 0; j < i; j++) {
-      if (!buf[j]) continue;
-      if (buf[i] < buf[j] + bytes[j] && buf[j] < buf[i] + bytes[i]) { h->err = "forward outputs overlap"; return 1; }
-    }
-  }
-  if (!any || n == 0) return 0;
+  if (buffers_overlap(buf, bytes, 5)) { h->err = "forward outputs overlap"; return 1; }
+  if (!(d_dof || d_body_acc || d_cfrc_int || d_cfrc_ext) || n == 0) return 0;
   CK(cudaSetDevice(h->device));
   const FwdOut o = {d_dof, d_body_acc, d_cfrc_int, d_cfrc_ext};
   cudaStream_t s = (cudaStream_t)stream;

@@ -2036,6 +2036,20 @@ LS_FN void make_constraint(const int ms, EnvS<C>& e) {
 // ----------------------------------------------------------------------------------------------------------
 // velocity-dependent smooth terms: comVel, RNE bias, passive, actuation -> qfrc_smooth, qacc_smooth
 // ----------------------------------------------------------------------------------------------------------
+// the force of actuator i at the env's state and e.ctrl, before the gear: ctrl clamped to its range, gain and bias, the
+// force clamped to its range. smooth_forces and forward_outputs' dof row both take it from here, so the dof outputs and
+// forward_dynamics' dof row agree bit for bit.
+template <class C>
+LS_DEV float actuator_force(const DevModel& m, const EnvS<C>& e, const int i) {
+  float c = e.ctrl[i];
+  if (m.actuator_ctrllimited[i]) c = fminf(m.actuator_ctrlrange[2 * i + 1], fmaxf(m.actuator_ctrlrange[2 * i], c));
+  const int d = m.actuator_dof[i];
+  float f = m.actuator_gain[i] * c + m.actuator_bias[3 * i] + m.actuator_bias[3 * i + 1] * e.qpos[d] +
+            m.actuator_bias[3 * i + 2] * e.qvel[d];
+  if (m.actuator_forcelimited[i]) f = fminf(m.actuator_forcerange[2 * i + 1], fmaxf(m.actuator_forcerange[2 * i], f));
+  return f;
+}
+
 // mj_comVel + mj_rne (bias forces) without tree recursion: all spatial vectors live in one frame (world-aligned, at the
 // CoM), so the velocity / bias acceleration of a body is a plain SUM over the dofs of its chain (bit mask
 // body_dofmask) and the force a dof feels is a plain sum over the bodies of its subtree. Three fully parallel passes.
@@ -2103,12 +2117,8 @@ LS_FN void smooth_forces(const int ms, EnvS<C>& e) {
   }
   SYNC();
   PAR_FOR(i, m.nu) {
-    float c = e.ctrl[i];
-    if (m.actuator_ctrllimited[i]) c = fminf(m.actuator_ctrlrange[2 * i + 1], fmaxf(m.actuator_ctrlrange[2 * i], c));
-    int d = m.actuator_dof[i];
-    float f = m.actuator_gain[i] * c + m.actuator_bias[3 * i] + m.actuator_bias[3 * i + 1] * e.qpos[d] +
-              m.actuator_bias[3 * i + 2] * e.qvel[d];
-    if (m.actuator_forcelimited[i]) f = fminf(m.actuator_forcerange[2 * i + 1], fmaxf(m.actuator_forcerange[2 * i], f));
+    const float f = actuator_force(m, e, i);     // (before the dof load: in the other order the step kernels' code changes)
+    const int d = m.actuator_dof[i];
     // one actuator per dof in all in-scope models -> no write conflict
     e.qfrc_smooth[d] += m.actuator_gear[i] * f;
     // dof outputs: the force of this evaluation, for dof_outputs after the integrator (not from a warp that shadows
@@ -2842,6 +2852,17 @@ LS_FN void forward(const int ms, EnvS<C>& e, const SolverOpts so) {
   fwd_constraint(ms, e, so);
 }
 
+// whether qpos or qvel is non-finite at any of the env's nv dofs, or `bad` (a caller's test of further entries, per lane)
+// is set on any lane: the same answer on every lane of the warp
+template <class C>
+LS_DEV bool nonfinite_state(const EnvS<C>& e, const int nv, bool bad = false) {
+  PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+#ifndef LS_EMULATE
+  bad = __any_sync(0xffffffffu, bad);
+#endif
+  return bad;
+}
+
 // ----------------------------------------------------------------------------------------------------------
 // inverse dynamics (locosim_inverse): MuJoCo 2.3.7's continuous-time mj_inverse
 // ----------------------------------------------------------------------------------------------------------
@@ -2908,11 +2929,8 @@ LS_FN void inverse_dynamics(const int ms, EnvS<C>& e, float* out) {
   const DevModel& m = c_models[ms];
   const int nv = m.nv;
   bool bad = false;
-  PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]) && isfinite(e.qacc[i]));
-#ifndef LS_EMULATE
-  bad = __any_sync(0xffffffffu, bad);
-#endif
-  if (bad) {
+  PAR_FOR(i, nv) bad |= !isfinite(e.qacc[i]);
+  if (nonfinite_state(e, nv, bad)) {
     PAR_FOR(i, nv) out[i] = 0.0f;
     SYNC();
     return;
@@ -2971,12 +2989,7 @@ template <class C>
 LS_FN void dynamics_terms(const int ms, EnvS<C>& e, const DynOut o) {
   const DevModel& m = c_models[ms];
   const int nv = m.nv, nb = m.nb;
-  bool bad = false;
-  PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
-#ifndef LS_EMULATE
-  bad = __any_sync(0xffffffffu, bad);
-#endif
-  if (bad) {
+  if (nonfinite_state(e, nv)) {
     if (o.M) PAR_FOR(k, nv * nv) o.M[k] = 0.0f;
     if (o.bias) PAR_FOR(k, nv) o.bias[k] = 0.0f;
     if (o.passive) PAR_FOR(k, nv) o.passive[k] = 0.0f;
@@ -3274,19 +3287,6 @@ struct FwdOut {
   float *dof, *body_acc, *cfrc_int, *cfrc_ext;
 };
 
-// the force of actuator i at the env's state and e.ctrl: smooth_forces' expression (before the gear), which stores the
-// force only while the dof outputs are registered and only inside a step
-template <class C>
-LS_DEV float actuator_force(const DevModel& m, const EnvS<C>& e, const int i) {
-  float c = e.ctrl[i];
-  if (m.actuator_ctrllimited[i]) c = fminf(m.actuator_ctrlrange[2 * i + 1], fmaxf(m.actuator_ctrlrange[2 * i], c));
-  const int d = m.actuator_dof[i];
-  float f = m.actuator_gain[i] * c + m.actuator_bias[3 * i] + m.actuator_bias[3 * i + 1] * e.qpos[d] +
-            m.actuator_bias[3 * i + 2] * e.qvel[d];
-  if (m.actuator_forcelimited[i]) f = fminf(m.actuator_forcerange[2 * i + 1], fmaxf(m.actuator_forcerange[2 * i], f));
-  return f;
-}
-
 // The outputs of the forward evaluation forward() has just made (the caller ran it at e.qpos / e.qvel / e.ctrl). In order:
 //   (1) the dof row: per dof the sum of gear * actuator_force over its actuators in actuator order, qfrc_constraint and
 //       qacc, read before anything below overwrites the storage they share with cinert / cdof_dot;
@@ -3434,12 +3434,8 @@ LS_FN void forward_dynamics(const int ms, EnvS<C>& e, const SolverOpts so, const
   const DevModel& m = c_models[ms];
   const int nv = m.nv, nb = m.nb, nu = m.nu;
   bool bad = false;
-  PAR_FOR(i, nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
   PAR_FOR(i, nu) bad |= !isfinite(e.ctrl[i]);
-#ifndef LS_EMULATE
-  bad = __any_sync(0xffffffffu, bad);
-#endif
-  if (bad) {
+  if (nonfinite_state(e, nv, bad)) {
     if (o.dof) PAR_FOR(k, nv * LS_DOF_DIM) o.dof[k] = 0.0f;
     if (o.body_acc) PAR_FOR(k, nb * LS_BODY_ACC_DIM) o.body_acc[k] = 0.0f;
     if (o.cfrc_int) PAR_FOR(k, nb * LS_CONTACT_DIM) o.cfrc_int[k] = 0.0f;

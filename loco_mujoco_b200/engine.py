@@ -5,6 +5,7 @@ There is NO CPU fallback: if the shared library is missing or no CUDA device is 
 raises. (The fp64 CPU oracle under oracle/ is test infrastructure and is never imported from here.)
 """
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -221,6 +222,31 @@ class CudaEngine:
         if rc != 0:
             raise RuntimeError("locosim: %s" % self.lib.locosim_last_error(self.h).decode())
 
+    def _check_tensor(self, x, name, shape):
+        """Refuse `x` (ValueError naming it) unless it is a contiguous float32 tensor on this engine's device of exactly
+        `shape`: the engine reads or writes every env's whole rows through its pointer. Anything without a tensor's
+        dtype / is_contiguous / device / shape (None, a numpy array) is refused as well."""
+        t = self.torch
+        if not all(hasattr(x, a) for a in ("dtype", "is_contiguous", "device", "shape")) or x.dtype != t.float32 \
+                or not x.is_contiguous() or x.device != self.device:
+            raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+        if tuple(x.shape) != shape:
+            raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+
+    @staticmethod
+    def _check_disjoint(spans):
+        """Refuse (ValueError naming both) any two of `spans` (name, tensor, shape) whose float32 buffers overlap; a None
+        tensor is skipped. Byte sizes come from the checked shapes."""
+        seen = []
+        for name, x, shape in spans:
+            if x is None:
+                continue
+            a, size = x.data_ptr(), 4 * math.prod(shape)
+            for other, b, bsize in seen:
+                if size and bsize and a < b + bsize and b < a + size:
+                    raise ValueError("%s and %s must not overlap" % (other, name))
+            seen.append((name, a, size))
+
     def _stream(self):
         return ctypes.c_void_p(self.torch.cuda.current_stream(self.device).cuda_stream)
 
@@ -258,10 +284,7 @@ class CudaEngine:
         engine's byte (bit 0 absorbing, bit 1 truncated by `set_time_limit`: `split_done`).
         packed: optional uint8 cuda buffer of `packed_bytes` (16-byte aligned, e.g. one time slot of a rollout buffer)
         the kernel writes this step's obs / reward / done into instead of the engine's own `packed_out`."""
-        if action.dtype != self.torch.float32 or not action.is_contiguous() or action.device != self.device:
-            raise ValueError("action must be a contiguous float32 tensor on %s" % self.device)
-        if tuple(action.shape) != (self.n_envs, self.action_dim):
-            raise ValueError("action shape %s != %s" % (tuple(action.shape), (self.n_envs, self.action_dim)))
+        self._check_tensor(action, "action", (self.n_envs, self.action_dim))
         if packed is None:
             obs, reward, done = self.obs, self.reward, self.done
         else:
@@ -284,9 +307,9 @@ class CudaEngine:
         return q, v, w
 
     def set_state(self, qpos, qvel, qacc_warmstart=None):
-        for x in (qpos, qvel, qacc_warmstart):
-            if x is not None and (x.dtype != self.torch.float32 or not x.is_contiguous()):
-                raise ValueError("state tensors must be contiguous float32")
+        for x, name in ((qpos, "qpos"), (qvel, "qvel"), (qacc_warmstart, "qacc_warmstart")):
+            if x is not None:
+                self._check_tensor(x, name, (self.n_envs, self.nq))
         self._check(self.lib.locosim_set_state(self.h, _ptr(qpos), _ptr(qvel), _ptr(qacc_warmstart), self._stream()))
 
     def set_time_limit(self, max_episode_steps=0, end_of_trajectory=False):
@@ -299,14 +322,9 @@ class CudaEngine:
         [n_envs, nbody, 6] (force then torque, world frame, at each body's centre of mass; body 0 ignored), `qfrc` float32
         cuda [n_envs, nq]; either None. The engine reads the tensors in every later step, zeroes the rows of every env it
         resets, and keeps a reference to them. None, None turns the feature off. Register outside of CUDA-graph capture."""
-        t = self.torch
         for x, shape, name in ((xfrc, (self.n_envs, self.nbody, 6), "xfrc"), (qfrc, (self.n_envs, self.nq), "qfrc")):
-            if x is None:
-                continue
-            if x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
-                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
-            if tuple(x.shape) != shape:
-                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+            if x is not None:
+                self._check_tensor(x, name, shape)
         self._check(self.lib.locosim_set_applied_forces(self.h, _ptr(xfrc), _ptr(qfrc)))
         self._applied = (xfrc, qfrc)
 
@@ -318,15 +336,9 @@ class CudaEngine:
         CUDA-graph capture, and capture a step again after turning the feature on: whether a step writes the rows is fixed
         when it is captured (a graph captured with nothing registered writes only the terminal rows of the envs it resets;
         one captured with buffers registered writes into whatever buffers are registered at each replay)."""
-        t = self.torch
-        shape = (self.n_envs, self.nbody, BODY_DIM)
         for x, name in ((body, "body"), (next_body, "next_body")):
-            if x is None:
-                continue
-            if x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
-                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
-            if tuple(x.shape) != shape:
-                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+            if x is not None:
+                self._check_tensor(x, name, (self.n_envs, self.nbody, BODY_DIM))
         self._check(self.lib.locosim_set_body_outputs(self.h, _ptr(body), _ptr(next_body)))
         self._body_out = (body, next_body)
         self.kernels_per_step = self.lib.locosim_kernels_per_step(self.h)     # (+1 while registered: body_kernel)
@@ -340,15 +352,9 @@ class CudaEngine:
         `next_ref` as well, set_state() does not. The engine keeps a reference to them. None, None turns the feature off.
         The CUDA-graph rules are those of set_body_outputs: register outside of capture and capture a step again after
         turning the feature on."""
-        t = self.torch
-        shape = (self.n_envs, self.nbody, BODY_DIM)
         for x, name in ((ref, "ref"), (next_ref, "next_ref")):
-            if x is None:
-                continue
-            if x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
-                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
-            if tuple(x.shape) != shape:
-                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
+            if x is not None:
+                self._check_tensor(x, name, (self.n_envs, self.nbody, BODY_DIM))
         self._check(self.lib.locosim_set_reference_outputs(self.h, _ptr(ref), _ptr(next_ref)))
         self._ref_out = (ref, next_ref)
         self.kernels_per_step = self.lib.locosim_kernels_per_step(self.h)     # (+1 while registered: body_kernel)
@@ -359,13 +365,8 @@ class CudaEngine:
         and torque about the body-frame origin that the body's contacts exert on it, averaged over the step's sub-steps
         (zeros for a non-finite env). reset() and set_state() leave it alone. The engine keeps a reference to it. Register
         outside of CUDA-graph capture; a step captured earlier writes the buffer registered when it is replayed."""
-        t = self.torch
         if contact is not None:
-            shape = (self.n_envs, self.nbody, CONTACT_DIM)
-            if contact.dtype != t.float32 or not contact.is_contiguous() or contact.device != self.device:
-                raise ValueError("contact must be a contiguous float32 tensor on %s" % self.device)
-            if tuple(contact.shape) != shape:
-                raise ValueError("contact shape %s != %s" % (tuple(contact.shape), shape))
+            self._check_tensor(contact, "contact", (self.n_envs, self.nbody, CONTACT_DIM))
         self._check(self.lib.locosim_set_contact_outputs(self.h, _ptr(contact)))
         self._contact_out = contact
 
@@ -375,13 +376,8 @@ class CudaEngine:
         force, the constraint force and the constrained acceleration, averaged over the step's sub-steps (zeros for a
         non-finite env). reset() and set_state() leave it alone. The engine keeps a reference to it. Register outside of
         CUDA-graph capture; a step captured earlier writes the buffer registered when it is replayed."""
-        t = self.torch
         if dof is not None:
-            shape = (self.n_envs, self.nq, DOF_DIM)
-            if dof.dtype != t.float32 or not dof.is_contiguous() or dof.device != self.device:
-                raise ValueError("dof must be a contiguous float32 tensor on %s" % self.device)
-            if tuple(dof.shape) != shape:
-                raise ValueError("dof shape %s != %s" % (tuple(dof.shape), shape))
+            self._check_tensor(dof, "dof", (self.n_envs, self.nq, DOF_DIM))
         self._check(self.lib.locosim_set_dof_outputs(self.h, _ptr(dof)))
         self._dof_out = dof
 
@@ -433,15 +429,9 @@ class CudaEngine:
         shape = (self.n_envs, self.nq)
         if out is None:
             out = t.empty(shape, dtype=t.float32, device=self.device)
-        for x, name in ((qacc, "qacc"), (out, "out")):
-            if not isinstance(x, t.Tensor) or x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
-                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
-            if tuple(x.shape) != shape:
-                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
-        nbytes = self.n_envs * self.nq * 4
-        a, b = qacc.data_ptr(), out.data_ptr()
-        if a < b + nbytes and b < a + nbytes:
-            raise ValueError("qacc and out must not overlap")
+        self._check_tensor(qacc, "qacc", shape)
+        self._check_tensor(out, "out", shape)
+        self._check_disjoint((("qacc", qacc, shape), ("out", out, shape)))
         self._check(self.lib.locosim_inverse(self.h, _ptr(qacc), _ptr(out), self._stream()))
         self.launches += 1
         return out
@@ -466,26 +456,13 @@ class CudaEngine:
         jacp rows), jac_com [n_envs, 3, nq] (mj_jacSubtreeCom of the robot). The tensors must not overlap. A non-finite
         state gives that env zero rows. Changes nothing else in the engine; stream-ordered, no allocation (can be captured
         in a CUDA graph). Returns {name: tensor} of the outputs given; with none given, launches nothing."""
-        t = self.torch
         n, nq = self.n_envs, self.nq
         outs = (("M", M, (n, nq, nq)), ("bias", bias, (n, nq)), ("passive", passive, (n, nq)), ("com", com, (n, COM_DIM)),
                 ("jac", jac, (n, self.nbody, 6, nq)), ("jac_com", jac_com, (n, 3, nq)))
-        spans = []
         for name, x, shape in outs:
-            if x is None:
-                continue
-            if not isinstance(x, t.Tensor) or x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
-                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
-            if tuple(x.shape) != shape:
-                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
-            size = 4
-            for k in shape:
-                size *= k
-            a = x.data_ptr()
-            for other, b, bsize in spans:
-                if size and bsize and a < b + bsize and b < a + size:
-                    raise ValueError("%s and %s must not overlap" % (name, other))
-            spans.append((name, a, size))
+            if x is not None:
+                self._check_tensor(x, name, shape)
+        self._check_disjoint(outs)
         given = {name: x for name, x, _ in outs if x is not None}
         if not given:
             return given
@@ -506,27 +483,14 @@ class CudaEngine:
         outputs given; with none given, launches nothing."""
         if action is None:
             raise ValueError("action is required")
-        t = self.torch
         n, nq, nb = self.n_envs, self.nq, self.nbody
         outs = (("action", action, (n, self.action_dim)), ("dof", dof, (n, nq, DOF_DIM)),
                 ("body_acc", body_acc, (n, nb, BODY_ACC_DIM)), ("cfrc_int", cfrc_int, (n, nb, CONTACT_DIM)),
                 ("cfrc_ext", cfrc_ext, (n, nb, CONTACT_DIM)))
-        spans = []
         for name, x, shape in outs:
-            if x is None:
-                continue
-            if not isinstance(x, t.Tensor) or x.dtype != t.float32 or not x.is_contiguous() or x.device != self.device:
-                raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
-            if tuple(x.shape) != shape:
-                raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
-            size = 4
-            for k in shape:
-                size *= k
-            a = x.data_ptr()
-            for other, b, bsize in spans:
-                if size and bsize and a < b + bsize and b < a + size:
-                    raise ValueError("%s and %s must not overlap" % (name, other))
-            spans.append((name, a, size))
+            if x is not None:
+                self._check_tensor(x, name, shape)
+        self._check_disjoint(outs)
         given = {name: x for name, x, _ in outs[1:] if x is not None}
         if not given:
             return given
@@ -537,8 +501,7 @@ class CudaEngine:
 
     def set_goal(self, goal):
         """goal: float32 cuda [n_envs, 4] per-episode goal features (A1: cos, sin, speed)."""
-        if goal.dtype != self.torch.float32 or not goal.is_contiguous() or tuple(goal.shape) != (self.n_envs, 4):
-            raise ValueError("goal must be a contiguous float32 [n_envs, 4] tensor")
+        self._check_tensor(goal, "goal", (self.n_envs, 4))
         self._check(self.lib.locosim_set_goal(self.h, _ptr(goal), self._stream()))
 
     def set_param_pool(self, pool):

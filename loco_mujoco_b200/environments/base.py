@@ -686,21 +686,13 @@ class LocoEnv:
         qvel layout (`dof_index(joint)`), body axes in the model's body order (`body_index(name)`). A non-finite state gives
         that env zero rows. `out`: the dict of an earlier call, filled in place and returned (a graph-captured loop then
         allocates nothing); terms it lacks are allocated. Changes nothing in the env."""
-        import torch
         eng = self._get_engine()
         n, nq = self.num_envs, self._model.nq
         shapes = dict(mass_matrix=(n, nq, nq), bias=(n, nq), passive=(n, nq), com=(n, 4),
                       body_jacobian=(n, self._model.nbody, 6, nq), com_jacobian=(n, 3, nq))
         want = dict(mass_matrix=mass_matrix, bias=bias, passive=passive, com=com, body_jacobian=body_jacobian,
                     com_jacobian=com_jacobian)
-        if out is None:
-            out = {}
-        elif not isinstance(out, dict):
-            raise ValueError("out must be the dict of an earlier dynamics_terms() call")
-        for k in self.DYNAMICS_TERMS:
-            if want[k] and out.get(k) is None:
-                out[k] = torch.empty(shapes[k], dtype=torch.float32, device=eng.device)
-        got = {k: out[k] if want[k] else None for k in self.DYNAMICS_TERMS}
+        out, got = self._query_outputs("dynamics_terms", self.DYNAMICS_TERMS, out, want, shapes, eng.device)
         eng.dynamics_terms(M=got["mass_matrix"], bias=got["bias"], passive=got["passive"], com=got["com"],
                            jac=got["body_jacobian"], jac_com=got["com_jacobian"])
         return out
@@ -730,21 +722,28 @@ class LocoEnv:
         non-finite state or action gives that env zero rows. `out`: the dict of an earlier call, filled in place and
         returned (a graph-captured loop then allocates nothing); outputs it lacks are allocated. Changes nothing in the env:
         the next step() is the same, bit for bit, as without this call."""
-        import torch
         eng = self._get_engine()
         n, nq, nb = self.num_envs, self._model.nq, self._model.nbody
         shapes = dict(dof=(n, nq, 3), body_acc=(n, nb, 6), cfrc_int=(n, nb, 6), cfrc_ext=(n, nb, 6))
         want = dict(dof=dof, body_acc=body_acc, cfrc_int=cfrc_int, cfrc_ext=cfrc_ext)
+        out, got = self._query_outputs("forward_dynamics", self.FORWARD_OUTPUTS, out, want, shapes, eng.device)
+        eng.forward(action, **got)
+        return out
+
+    @staticmethod
+    def _query_outputs(method, names, out, want, shapes, device):
+        """(out, got) of a query with the outputs `names`: `out` is the dict of an earlier `method` call, or None for a new
+        one; every output k asked for (want[k] true) that it lacks is allocated into it, float32 of shapes[k] on `device`.
+        got[k] is out[k] when asked for, else None."""
+        import torch
         if out is None:
             out = {}
         elif not isinstance(out, dict):
-            raise ValueError("out must be the dict of an earlier forward_dynamics() call")
-        for k in self.FORWARD_OUTPUTS:
+            raise ValueError("out must be the dict of an earlier %s() call" % method)
+        for k in names:
             if want[k] and out.get(k) is None:
-                out[k] = torch.empty(shapes[k], dtype=torch.float32, device=eng.device)
-        got = {k: out[k] if want[k] else None for k in self.FORWARD_OUTPUTS}
-        eng.forward(action, **got)
-        return out
+                out[k] = torch.empty(shapes[k], dtype=torch.float32, device=device)
+        return out, {k: out[k] if want[k] else None for k in names}
 
     # ---------------------------------------------------------------------------------------------------
     # the hot path

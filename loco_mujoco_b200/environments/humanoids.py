@@ -248,6 +248,14 @@ class HumanoidTorque4Ages(BaseHumanoid):
         return HumanoidTorque4Ages._generate4(task, mode, dataset_type, **kwargs)
 
 
+def _unavailable(feature):
+    """A method (or property getter) of HumanoidTorque4AgesAll that refuses `feature`."""
+    def refuse(self, *args, **kwargs):
+        raise NotImplementedError("%s are not available for HumanoidTorque4Ages mode 'all': use the single-scaling envs "
+                                  "(HumanoidTorque4Ages.<task>.<1-4>)" % feature)
+    return refuse
+
+
 class HumanoidTorque4AgesAll:
     """HumanoidTorque4Ages, mode "all" (base_humanoid_4_ages.py:28-105,107-150; humanoids.py:855-892): at the beginning of each
     episode one of the four humanoids (scalings 0.4 / 0.6 / 0.8 / 1.0) is drawn, then a start state from THAT humanoid's
@@ -291,70 +299,20 @@ class HumanoidTorque4AgesAll:
     def dt(self):
         return self.subs[0].dt
 
-    # ---- applied forces: the four humanoids differ in their bodies and the envs are interleaved over four engines ----
-    def _no_applied_forces(self, *args):
-        raise NotImplementedError("applied forces (xfrc_applied / qfrc_applied / body_index) are not available for "
-                                  "HumanoidTorque4Ages mode 'all': use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
-
-    xfrc_applied = property(_no_applied_forces)
-    qfrc_applied = property(_no_applied_forces)
-    body_index = _no_applied_forces
-
-    # ---- body outputs: for the same reason ----
-    def _no_body_outputs(self, *args):
-        raise NotImplementedError("body outputs (body_state / next_body_state) are not available for HumanoidTorque4Ages "
-                                  "mode 'all': use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
-
-    body_state = property(_no_body_outputs)
-    next_body_state = property(_no_body_outputs)
-
-    # ---- contact outputs: likewise ----
-    def _no_contact_outputs(self, *args):
-        raise NotImplementedError("contact outputs (contact_wrench) are not available for HumanoidTorque4Ages mode 'all': "
-                                  "use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
-
-    contact_wrench = property(_no_contact_outputs)
-
-    # ---- dof outputs: likewise ----
-    def _no_dof_outputs(self, *args):
-        raise NotImplementedError("dof outputs (dof_outputs) are not available for HumanoidTorque4Ages mode 'all': "
-                                  "use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
-
-    dof_outputs = property(_no_dof_outputs)
-
-    # ---- reference outputs: likewise ----
-    def _no_reference_outputs(self, *args):
-        raise NotImplementedError("reference outputs (reference_body_state / next_reference_body_state / "
-                                  "create_dataset_bodies) are not available for HumanoidTorque4Ages mode 'all': use the "
-                                  "single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
-
-    reference_body_state = property(_no_reference_outputs)
-    next_reference_body_state = property(_no_reference_outputs)
-    create_dataset_bodies = _no_reference_outputs
-
-    # ---- inverse dynamics: likewise ----
-    def _no_inverse_dynamics(self, *args):
-        raise NotImplementedError("inverse dynamics (inverse_dynamics / create_dataset_inverse / dof_index) is not available "
-                                  "for HumanoidTorque4Ages mode 'all': use the single-scaling envs "
-                                  "(HumanoidTorque4Ages.<task>.<1-4>)")
-
-    inverse_dynamics = _no_inverse_dynamics
-    create_dataset_inverse = _no_inverse_dynamics
-    dof_index = _no_inverse_dynamics
-
-    # ---- dynamics terms: likewise ----
-    def _no_dynamics_terms(self, *args, **kwargs):
-        raise NotImplementedError("the dynamics terms (dynamics_terms) are not available for HumanoidTorque4Ages mode 'all': "
-                                  "use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
-
-    dynamics_terms = _no_dynamics_terms
-
-    # ---- forward dynamics: likewise ----
-    def _no_forward_dynamics(self, *args, **kwargs):
-        raise NotImplementedError("the forward dynamics (forward_dynamics) are not available for HumanoidTorque4Ages mode "
-                                  "'all': use the single-scaling envs (HumanoidTorque4Ages.<task>.<1-4>)")
-
-    forward_dynamics = _no_forward_dynamics
+    # ---- the per-env outputs and the dynamics queries: the four humanoids differ in their bodies and the envs are
+    # interleaved over four engines ----
+    body_index = _unavailable("applied forces (xfrc_applied / qfrc_applied / body_index)")
+    xfrc_applied = qfrc_applied = property(body_index)
+    body_state = next_body_state = property(_unavailable("body outputs (body_state / next_body_state)"))
+    contact_wrench = property(_unavailable("contact outputs (contact_wrench)"))
+    dof_outputs = property(_unavailable("dof outputs (dof_outputs)"))
+    create_dataset_bodies = _unavailable("reference outputs (reference_body_state / next_reference_body_state / "
+                                         "create_dataset_bodies)")
+    reference_body_state = next_reference_body_state = property(create_dataset_bodies)
+    inverse_dynamics = create_dataset_inverse = dof_index = _unavailable(
+        "inverse dynamics (inverse_dynamics / create_dataset_inverse / dof_index)")
+    dynamics_terms = _unavailable("the dynamics terms (dynamics_terms)")
+    forward_dynamics = _unavailable("the forward dynamics (forward_dynamics)")
 
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""
