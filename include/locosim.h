@@ -345,6 +345,62 @@ int locosim_dynamics_terms(locosim_t* h, float* d_M, float* d_bias, float* d_pas
 int locosim_forward(locosim_t* h, const float* d_action, float* d_dof, float* d_body_acc, float* d_cfrc_int,
                     float* d_cfrc_ext, void* stream);
 
+/* Saved simulation states, MuJoCo's mj_copyData for a batch: every env's whole state as one int32 row of
+ * locosim_state_words() words on the device, to be loaded back into the same env or into any other env of a handle with the
+ * same layout tag (forks for sampling-based MPC, reset-to-state curricula, replays).
+ *
+ * Row layout (the words are fp32 bits where the field is fp32; nv = locosim_nq, D = locosim_obs_dim):
+ *   LS_STATE_TAG      2 words: LS_STATE_VERSION, then a fingerprint of nv, nbody, obs_dim, n_goal, n_traj and traj_len
+ *                     computed when the handle is created. Two handles of one task (shards, MixedBatch members) share it.
+ *   LS_STATE_EPISODE  the reset counter: the number of the env's next reset in its counter-based random stream
+ *   LS_STATE_DR_ROW   the parameter-pool row (domain-randomisation draw; carry tasks: the carried weight)
+ *   LS_STATE_CURSOR   the trajectory cursor traj * traj_len + sample (locosim_get_cursor)
+ *   LS_STATE_ANGLE    fp32: the setup_random_rot angle of the running episode (0 without the option)
+ *   LS_STATE_EP       4 words: length, return (fp32), last length, last return (fp32) (locosim_get_episode_stats)
+ *   LS_STATE_GOAL     4 words (fp32): the goal features (locosim_set_goal)
+ *   LS_STATE_QPOS(nv), LS_STATE_QVEL(nv), LS_STATE_WARMSTART(nv)   nv words each (fp32): locosim_get_state
+ *   LS_STATE_OBS(nv)  D words (fp32): the observation the env acts on next
+ *   then zeros up to LS_STATE_WORDS(nv, D), a multiple of 4.
+ *
+ * locosim_save_state writes one row per env into d_state int32 [n_envs, W]. d_obs fp32 [n_envs, obs_dim] is required: the
+ * observation the env acts on next, i.e. a step's d_next_obs or a reset's d_obs. (The foot-force part of an observation is
+ * the mean over the last step's sub-steps, which the engine does not keep after the step.)
+ *
+ * locosim_load_state: env i takes row d_row[i] of the n_rows rows of d_state int32 [n_rows, W]; d_row int32 [n_envs], or
+ * NULL for row i (then n_rows must equal n_envs). n_rows may be smaller or larger than n_envs. An env whose index is
+ * negative or >= n_rows, or whose row carries another layout tag, is left untouched (nothing can be reported from the
+ * device without a synchronisation). A loaded env gets every field above back; its pool row is clamped into the current
+ * parameter pool and its cursor into the trajectory table (a row saved before a smaller locosim_set_param_pool cannot index
+ * out of bounds). Its rotation angle is pinned to its episode, so that its reference rows use the saved angle rather than
+ * the one drawn for the destination env. The stored observation goes to d_obs fp32 [n_envs, obs_dim] (may be NULL; the
+ * rows of envs not loaded are not written). With body or reference outputs registered, d_next_body, the reference keys and
+ * d_next_ref of the loaded envs are rewritten as locosim_reset_rows writes them (one more kernel).
+ * Not part of a row, and left alone by a load: the diagnostic counters (locosim_get_counters; also the regrouping key,
+ * which changes no bit of any result), the caller's applied-force buffers (index them with the same rows), and the
+ * handle-wide settings (solver, time limit, parameter pool, registered outputs).
+ * A loaded env keeps its own global env id: its next reset draws (traj, sample), the pool row and the rotation angle from
+ * the destination's stream at the saved reset counter. Loading a row back into the env it was saved from therefore
+ * replays the original bit for bit, auto-resets included, on any launch path; envs forked from one row are identical
+ * until their first reset and then diverge.
+ * Both calls are stream-ordered, synchronise nothing and allocate nothing: they can be captured in a CUDA graph. d_state
+ * must be 16-byte aligned and must not overlap d_obs (or d_row); both are refused. */
+#define LS_STATE_VERSION 0x4C530001
+#define LS_STATE_TAG 0
+#define LS_STATE_EPISODE 2
+#define LS_STATE_DR_ROW 3
+#define LS_STATE_CURSOR 4
+#define LS_STATE_ANGLE 5
+#define LS_STATE_EP 8
+#define LS_STATE_GOAL 12
+#define LS_STATE_QPOS(nv) (16)
+#define LS_STATE_QVEL(nv) (16 + (nv))
+#define LS_STATE_WARMSTART(nv) (16 + 2 * (nv))
+#define LS_STATE_OBS(nv) (16 + 3 * (nv))
+#define LS_STATE_WORDS(nv, obs_dim) ((16 + 3 * (nv) + (obs_dim) + 3) / 4 * 4)
+int locosim_state_words(const locosim_t* h);
+int locosim_save_state(locosim_t* h, const float* d_obs, int32_t* d_state, void* stream);
+int locosim_load_state(locosim_t* h, const int32_t* d_state, int n_rows, const int32_t* d_row, float* d_obs, void* stream);
+
 /* Per-episode goal features (UnitreeA1: cos / sin of the goal direction and the goal speed, GoalDirectionVelocity set in
  * setup() unitreeA1.py:287-291); normally loaded from the reset table, settable for reset(obs=...) (base.py:217-218,633-654).
  * d_goal fp32 [n_envs, 4]. */

@@ -132,6 +132,86 @@ __global__ void reset_kernel(int ms, DevTask t, EngineState st, const uint8_t* m
     if (st.rot_angle && t.rot[0] >= 0) rot_pin[env] = make_int2(ep + 1, __float_as_int(angle));   // (episode_angle)
   }
 }
+
+// ----------------------------------------------------------------------------------------------------------
+// saved states (locosim_save_state / locosim_load_state, row layout LS_STATE_* of include/locosim.h): one warp per env, the
+// row moved as 16-byte words. Words 0-15 are four int4: (tag, tag, episode, pool row), (cursor, angle, 0, 0), the episode
+// statistics, the goal; from LS_STATE_QPOS on the per-dof arrays and the observation follow word by word.
+// ----------------------------------------------------------------------------------------------------------
+// word k (>= 0) of an env's row after LS_STATE_QPOS
+__device__ __forceinline__ int state_array_word(const EngineState& st, const float* __restrict__ obs, int env, int nv, int D,
+                                                int k) {
+  if (k < nv) return __float_as_int(st.qpos[(size_t)env * nv + k]);
+  if ((k -= nv) < nv) return __float_as_int(st.qvel[(size_t)env * nv + k]);
+  if ((k -= nv) < nv) return __float_as_int(st.ws[(size_t)env * nv + k]);
+  if ((k -= nv) < D) return __float_as_int(obs[(size_t)env * D + k]);
+  return 0;
+}
+__device__ __forceinline__ void state_array_store(const EngineState& st, float* __restrict__ obs, int env, int nv, int D, int k,
+                                                  int w) {
+  if (k < nv) st.qpos[(size_t)env * nv + k] = __int_as_float(w);
+  else if ((k -= nv) < nv) st.qvel[(size_t)env * nv + k] = __int_as_float(w);
+  else if ((k -= nv) < nv) st.ws[(size_t)env * nv + k] = __int_as_float(w);
+  else if ((k -= nv) < D) { if (obs) obs[(size_t)env * D + k] = __int_as_float(w); }
+}
+
+__global__ void save_state_kernel(DevTask t, EngineState st, const float* __restrict__ obs, int4* __restrict__ rows,
+                                  int n_envs, int nv, int words, int fingerprint, uint64_t seed, int64_t env_off,
+                                  const int2* __restrict__ rot_pin) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= n_envs) return;
+  const int nc = words / 4, D = t.obs_dim;
+  int4* row = rows + (size_t)env * nc;
+  for (int c = lane; c < nc; c += 32) {
+    int4 v;
+    if (c == 0) v = make_int4(LS_STATE_VERSION, fingerprint, st.episode[env], st.dr_row[env]);
+    else if (c == 1) {
+      const float angle = episode_angle(t, rot_pin, seed, env_off + env, env, st.episode[env]);
+      v = make_int4(st.cursor[env], __float_as_int(angle), 0, 0);
+    } else if (c == 2) v = st.ep[env];
+    else if (c == 3) v = reinterpret_cast<const int4*>(st.goal)[env];
+    else {
+      const int k = 4 * c - LS_STATE_QPOS(nv);
+      v = make_int4(state_array_word(st, obs, env, nv, D, k), state_array_word(st, obs, env, nv, D, k + 1),
+                    state_array_word(st, obs, env, nv, D, k + 2), state_array_word(st, obs, env, nv, D, k + 3));
+    }
+    row[c] = v;
+  }
+}
+
+// env i <- row idx[i] (idx NULL: row i); loaded[i] = whether it was (the mask of the body / reference rows written next)
+__global__ void load_state_kernel(DevTask t, EngineState st, const int4* __restrict__ rows, int n_rows,
+                                  const int* __restrict__ idx, float* __restrict__ obs, int n_envs, int nv, int words,
+                                  int fingerprint, int2* __restrict__ rot_pin, int* __restrict__ reset_mark,
+                                  uint8_t* __restrict__ loaded) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= n_envs) return;
+  const int nc = words / 4, D = t.obs_dim;
+  const int r = idx ? idx[env] : env;
+  bool ok = r >= 0 && r < n_rows;
+  const int4* row = rows + (size_t)(ok ? r : 0) * nc;
+  const int4 h0 = ok ? row[0] : make_int4(0, 0, 0, 0);
+  ok = ok && h0.x == LS_STATE_VERSION && h0.y == fingerprint;
+  if (lane == 0) loaded[env] = ok ? 1 : 0;
+  if (!ok) return;
+  for (int c = lane; c < nc; c += 32) {
+    const int4 v = row[c];
+    if (c == 0) {
+      st.episode[env] = v.z;
+      st.dr_row[env] = min(max(v.w, 0), st.pool_K - 1);
+    } else if (c == 1) {
+      st.cursor[env] = min(max(v.x, 0), t.n_traj * t.traj_len - 1);
+      rot_pin[env] = make_int2(h0.z, v.y);          // (episode_angle: the saved angle, not the destination's draw)
+    } else if (c == 2) st.ep[env] = v;
+    else if (c == 3) reinterpret_cast<int4*>(st.goal)[env] = v;
+    else {
+      const int k = 4 * c - LS_STATE_QPOS(nv);
+      state_array_store(st, obs, env, nv, D, k, v.x); state_array_store(st, obs, env, nv, D, k + 1, v.y);
+      state_array_store(st, obs, env, nv, D, k + 2, v.z); state_array_store(st, obs, env, nv, D, k + 3, v.w);
+    }
+  }
+  if (lane == 0 && reset_mark) reset_mark[env] = 0;
+}
 #endif
 
 // ----------------------------------------------------------------------------------------------------------
@@ -1122,6 +1202,8 @@ struct locosim_handle {
   DevRefOut refout = {nullptr, nullptr, nullptr};
   int4* ref_key = nullptr;           // the reference keys [n_envs] (DevRefOut::key) once reference outputs were registered
   int2* rot_pin = nullptr;           // [n_envs] episode number and angle of the last rotation reset_kernel was given (episode_angle)
+  uint8_t* load_mask = nullptr;      // [n_envs] the envs the last locosim_load_state loaded (load_state_kernel -> body_kernel)
+  int state_fp = 0;                  // layout fingerprint of the saved-state rows (LS_STATE_TAG)
   float* d_model_row = nullptr;      // the compiled model's own parameter row (locosim_create_dataset_bodies), on first use
   DevContact contact = {nullptr, 1};
   DevDof dof = {nullptr, 1};
@@ -1483,12 +1565,20 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
        cudaMalloc((void**)&h->st.dr_row, N * 4) == cudaSuccess && cudaMalloc((void**)&h->st.perm, N * 4) == cudaSuccess &&
        cudaMalloc((void**)&h->st.cursor, N * 4) == cudaSuccess &&
        cudaMalloc((void**)&h->st.ep, N * 16) == cudaSuccess && cudaMalloc((void**)&h->rot_pin, N * 8) == cudaSuccess &&
+       cudaMalloc((void**)&h->load_mask, N) == cudaSuccess &&
        up((void**)&h->d_pool, h->hm.default_row.data(), h->hm.default_row.size() * 4);
   if (!ok) { std::string m = std::string("device allocation failed: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); g_create_error = m; return 1; }
   cudaMemset(h->st.qpos, 0, N * nv * 4); cudaMemset(h->st.qvel, 0, N * nv * 4); cudaMemset(h->st.ws, 0, N * nv * 4);
   cudaMemset(h->st.goal, 0, N * 16); cudaMemset(h->st.episode, 0, N * 4); cudaMemset(h->st.counters, 0, N * 32);
   cudaMemset(h->st.dr_row, 0, N * 4); cudaMemset(h->st.cursor, 0, N * 4);
-  cudaMemset(h->st.ep, 0, N * 16); cudaMemset(h->rot_pin, 0, N * 8);
+  cudaMemset(h->st.ep, 0, N * 16); cudaMemset(h->rot_pin, 0, N * 8); cudaMemset(h->load_mask, 0, N);
+  {
+    // FNV-1a over what the row layout and its indices depend on
+    const int dims[7] = {LS_STATE_VERSION, h->hm.nv, h->hm.nb, h->ht.obs_dim, h->ht.n_goal, h->ht.n_traj, h->ht.traj_len};
+    uint32_t f = 2166136261u;
+    for (int d : dims) for (int b = 0; b < 4; b++) { f ^= ((uint32_t)d >> (8 * b)) & 255u; f *= 16777619u; }
+    h->state_fp = (int)f;
+  }
   h->st.max_episode_steps = 0; h->st.end_of_trajectory = 0;
   h->st.rot_angle = nullptr;
   { std::vector<int> id(N); for (size_t i = 0; i < N; i++) id[i] = (int)i; cudaMemcpy(h->st.perm, id.data(), N * 4, cudaMemcpyHostToDevice); }
@@ -1539,7 +1629,7 @@ void locosim_destroy(locosim_t* h) {
   cudaFree(h->split.carry); cudaFree(h->split.bcount); cudaFree(h->split.benv); cudaFree(h->split.seq);
   cudaFree(h->pq.carry); cudaFree(h->pq.cnt); cudaFree(h->pq.tot); cudaFree(h->pq.benv); cudaFree(h->pq.seq);
   cudaFree(h->bodyout.reset_mark);
-  cudaFree(h->ref_key); cudaFree(h->rot_pin); cudaFree(h->d_model_row);
+  cudaFree(h->ref_key); cudaFree(h->rot_pin); cudaFree(h->load_mask); cudaFree(h->d_model_row);
   cudaFree(h->dof_act);
   delete h;
 }
@@ -1816,6 +1906,39 @@ int locosim_set_state(locosim_t* h, const float* q, const float* v, const float*
   if (w) CK(cudaMemcpyAsync(h->st.ws, w, bytes, cudaMemcpyDeviceToDevice, s));
   else CK(cudaMemsetAsync(h->st.ws, 0, bytes, s));
   return next_body_rows(h, nullptr, 1, s);
+}
+int locosim_state_words(const locosim_t* h) { return LS_STATE_WORDS(h->hm.nv, h->ht.obs_dim); }
+int locosim_save_state(locosim_t* h, const float* d_obs, int32_t* d_state, void* stream) {
+  if (!d_obs || !d_state) { h->err = "null buffer (save_state needs the observation the envs act on next)"; return 1; }
+  const size_t n = (size_t)h->n_envs;
+  const void* const buf[2] = {d_obs, d_state};
+  const size_t bytes[2] = {n * h->ht.obs_dim * 4, n * locosim_state_words(h) * 4};
+  if (buffers_overlap(buf, bytes, 2)) { h->err = "observation and state rows overlap"; return 1; }
+  if ((uintptr_t)d_state % 16) { h->err = "state rows must be 16-byte aligned"; return 1; }
+  CK(cudaSetDevice(h->device));
+  const int threads = 128, blocks = (h->n_envs * 32 + threads - 1) / threads;
+  save_state_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(h->dt, h->st, d_obs, reinterpret_cast<int4*>(d_state),
+                                                                  h->n_envs, h->hm.nv, locosim_state_words(h), h->state_fp,
+                                                                  h->seed, h->env_off, h->rot_pin);
+  CK(cudaGetLastError());
+  return 0;
+}
+int locosim_load_state(locosim_t* h, const int32_t* d_state, int n_rows, const int32_t* d_row, float* d_obs, void* stream) {
+  if (!d_state || n_rows < 1) { h->err = "no state rows"; return 1; }
+  if (!d_row && n_rows != h->n_envs) { h->err = "load_state without row indices needs one row per env"; return 1; }
+  const size_t n = (size_t)h->n_envs;
+  const void* const buf[3] = {d_state, d_row, d_obs};
+  const size_t bytes[3] = {(size_t)n_rows * locosim_state_words(h) * 4, n * 4, n * h->ht.obs_dim * 4};
+  if (buffers_overlap(buf, bytes, 3)) { h->err = "state rows, row indices and observation overlap"; return 1; }
+  if ((uintptr_t)d_state % 16) { h->err = "state rows must be 16-byte aligned"; return 1; }
+  CK(cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int threads = 128, blocks = (h->n_envs * 32 + threads - 1) / threads;
+  load_state_kernel<<<blocks, threads, 0, s>>>(h->dt, h->st, reinterpret_cast<const int4*>(d_state), n_rows, d_row, d_obs,
+                                               h->n_envs, h->hm.nv, locosim_state_words(h), h->state_fp, h->rot_pin,
+                                               h->bodyout.reset_mark, h->load_mask);
+  CK(cudaGetLastError());
+  return next_body_rows(h, h->load_mask, 7, s);
 }
 int locosim_set_goal(locosim_t* h, const float* g, void* stream) {
   if (!g) { h->err = "null buffer"; return 1; }

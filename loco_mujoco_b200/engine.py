@@ -101,6 +101,12 @@ def load_library():
     lib.locosim_dynamics_terms.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     lib.locosim_forward.restype = ip
     lib.locosim_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.locosim_state_words.restype = ip
+    lib.locosim_state_words.argtypes = [vp]
+    lib.locosim_save_state.restype = ip
+    lib.locosim_save_state.argtypes = [vp, vp, vp, vp]
+    lib.locosim_load_state.restype = ip
+    lib.locosim_load_state.argtypes = [vp, vp, ip, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -115,7 +121,8 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_get_episode_stats", "locosim_nbody", "locosim_set_applied_forces",
                     "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs",
                     "locosim_set_reference_outputs", "locosim_create_dataset_bodies", "locosim_inverse",
-                    "locosim_create_dataset_inverse", "locosim_dynamics_terms", "locosim_forward"]
+                    "locosim_create_dataset_inverse", "locosim_dynamics_terms", "locosim_forward", "locosim_state_words",
+                    "locosim_save_state", "locosim_load_state"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -129,6 +136,16 @@ COM_DIM = 4
 # values per body row of the forward dynamics' body accelerations (include/locosim.h LS_BODY_ACC_DIM): angular acceleration
 # (3), linear acceleration of the body-frame origin minus gravity (3), world frame
 BODY_ACC_DIM = 6
+
+
+
+def state_layout(nq, obs_dim):
+    """{field: (offset, length)} of a saved-state row (include/locosim.h LS_STATE_*), int32 words; "words" is the row length
+    W. Fields stored as fp32 (angle, ep[1], ep[3], goal, qpos, qvel, qacc_warmstart, obs) are read with `.view(float32)`."""
+    return dict(tag=(0, 2), episode=(2, 1), dr_row=(3, 1), cursor=(4, 1), angle=(5, 1), ep=(8, 4), goal=(12, 4),
+                qpos=(16, nq), qvel=(16 + nq, nq), qacc_warmstart=(16 + 2 * nq, nq), obs=(16 + 3 * nq, obs_dim),
+                words=(0, (16 + 3 * nq + obs_dim + 3) // 4 * 4))
+
 
 # bits of the done byte of a step (include/locosim.h)
 DONE_ABSORBING, DONE_TRUNCATED = 1, 2
@@ -211,6 +228,7 @@ class CudaEngine:
         self.next_obs = torch.zeros((n_envs, self.obs_dim), dtype=torch.float32, device=self.device)
         self.launches = 0
         self.kernels_per_step = self.lib.locosim_kernels_per_step(h)
+        self.state_words = self.lib.locosim_state_words(h)
 
     def views_of(self, packed):
         """(obs [N, D] f32, reward [N] f32, done [N] u8) views of a buffer laid out like `packed_out`."""
@@ -222,21 +240,21 @@ class CudaEngine:
         if rc != 0:
             raise RuntimeError("locosim: %s" % self.lib.locosim_last_error(self.h).decode())
 
-    def _check_tensor(self, x, name, shape):
-        """Refuse `x` (ValueError naming it) unless it is a contiguous float32 tensor on this engine's device of exactly
-        `shape`: the engine reads or writes every env's whole rows through its pointer. Anything without a tensor's
-        dtype / is_contiguous / device / shape (None, a numpy array) is refused as well."""
+    def _check_tensor(self, x, name, shape, dtype="float32"):
+        """Refuse `x` (ValueError naming it) unless it is a contiguous tensor of `dtype` (float32 or int32) on this
+        engine's device of exactly `shape`: the engine reads or writes every env's whole rows through its pointer. Anything
+        without a tensor's dtype / is_contiguous / device / shape (None, a numpy array) is refused as well."""
         t = self.torch
-        if not all(hasattr(x, a) for a in ("dtype", "is_contiguous", "device", "shape")) or x.dtype != t.float32 \
+        if not all(hasattr(x, a) for a in ("dtype", "is_contiguous", "device", "shape")) or x.dtype != getattr(t, dtype) \
                 or not x.is_contiguous() or x.device != self.device:
-            raise ValueError("%s must be a contiguous float32 tensor on %s" % (name, self.device))
+            raise ValueError("%s must be a contiguous %s tensor on %s" % (name, dtype, self.device))
         if tuple(x.shape) != shape:
             raise ValueError("%s shape %s != %s" % (name, tuple(x.shape), shape))
 
     @staticmethod
     def _check_disjoint(spans):
-        """Refuse (ValueError naming both) any two of `spans` (name, tensor, shape) whose float32 buffers overlap; a None
-        tensor is skipped. Byte sizes come from the checked shapes."""
+        """Refuse (ValueError naming both) any two of `spans` (name, tensor, shape) whose float32 or int32 buffers overlap; a
+        None tensor is skipped. Byte sizes come from the checked shapes."""
         seen = []
         for name, x, shape in spans:
             if x is None:
@@ -498,6 +516,53 @@ class CudaEngine:
                                              self._stream()))
         self.launches += 1
         return given
+
+    @property
+    def state_layout(self):
+        """{field: (offset, length)} of a saved-state row (`state_layout(nq, obs_dim)`)."""
+        return state_layout(self.nq, self.obs_dim)
+
+    def save_state(self, obs, out=None):
+        """Save every env's whole state (include/locosim.h locosim_save_state): int32 cuda [n_envs, state_words], one row per
+        env (`state_layout`), written into `out` (or a new tensor) and returned. `obs` float32 cuda [n_envs, obs_dim] is the
+        observation the envs act on next (a step's next_obs, a reset's observation); it is stored in the row. Stream-ordered,
+        no allocation when `out` is given (can be captured in a CUDA graph)."""
+        t = self.torch
+        shape = (self.n_envs, self.state_words)
+        if out is None:
+            out = t.empty(shape, dtype=t.int32, device=self.device)
+        self._check_tensor(obs, "obs", (self.n_envs, self.obs_dim))
+        self._check_tensor(out, "out", shape, "int32")
+        self._check_disjoint((("obs", obs, (self.n_envs, self.obs_dim)), ("out", out, shape)))
+        self._check(self.lib.locosim_save_state(self.h, _ptr(obs), _ptr(out), self._stream()))
+        self.launches += 1
+        return out
+
+    def load_state(self, rows, index=None, obs_out=None):
+        """Load saved states (include/locosim.h locosim_load_state): env i takes row index[i] of `rows` int32 cuda
+        [M, state_words] (M >= 1, any size); `index` int32 cuda [n_envs], or None for row i (then M must be n_envs). An env
+        whose index is negative or >= M, or whose row comes from an engine of another layout, is left untouched. The stored
+        observations of the loaded envs are written into `obs_out` float32 cuda [n_envs, obs_dim] if given (other rows are
+        not written). With body or reference outputs registered, their next-state rows of the loaded envs are rewritten
+        (one more kernel). Stream-ordered, no allocation (can be captured in a CUDA graph)."""
+        n, W, D = self.n_envs, self.state_words, self.obs_dim
+        rshape = tuple(getattr(rows, "shape", ()))
+        m = rshape[0] if len(rshape) == 2 and rshape[0] >= 1 else 1
+        self._check_tensor(rows, "rows", (m, W), "int32")
+        spans = [("rows", rows, (m, W))]
+        if index is None:
+            if m != n:
+                raise ValueError("rows must have one row per env (%d) when no index is given, not %d" % (n, m))
+        else:
+            self._check_tensor(index, "index", (n,), "int32")
+            spans.append(("index", index, (n,)))
+        if obs_out is not None:
+            self._check_tensor(obs_out, "obs_out", (n, D))
+            spans.append(("obs_out", obs_out, (n, D)))
+        self._check_disjoint(spans)
+        self._check(self.lib.locosim_load_state(self.h, _ptr(rows), m, _ptr(index), _ptr(obs_out), self._stream()))
+        self.launches += 1 if self._body_out[1] is None and self._ref_out == (None, None) else 2
+        return obs_out
 
     def set_goal(self, goal):
         """goal: float32 cuda [n_envs, 4] per-episode goal features (A1: cos, sin, speed)."""

@@ -746,6 +746,51 @@ class LocoEnv:
         return out, {k: out[k] if want[k] else None for k in names}
 
     # ---------------------------------------------------------------------------------------------------
+    # saved states (MuJoCo's mj_copyData for a batch, include/locosim.h locosim_save_state / locosim_load_state)
+    # ---------------------------------------------------------------------------------------------------
+    def save_state(self, out=None):
+        """Every env's whole simulation state as one int32 torch tensor [num_envs, W] on the env's device, one row per env:
+        qpos, qvel, the solver's warm start, the goal, the reset counter of the env's random stream, its parameter-pool row
+        (domain randomisation, the carried weight), trajectory cursor, episode length and return, rotation angle, and the
+        observation it acts on next (`engine.state_layout(nq, obs_dim)` names the words). `out`: a tensor of an earlier call,
+        filled in place (a graph-captured loop then allocates nothing). Rows load into any env of an env of the same task
+        (`load_state`); this env's shards and MixedBatch members included. Call after reset()."""
+        if self._obs is None:
+            raise RuntimeError("save_state() before the first reset(): there is no state to save")
+        eng = self._get_engine()
+        return eng.save_state(self._obs_tensor(eng), out)
+
+    def load_state(self, state, index=None):
+        """Put envs back into saved states: env i takes row index[i] of `state` (int32 [M, W] from `save_state`, any M;
+        `index` int32 [num_envs] on the env's device, or None for row i, then M must be num_envs). A negative index, one
+        >= M, or a row saved by an env of another task leaves the env untouched. Returns the observation to act on next,
+        as reset() does (untouched envs' rows unchanged). Loading a row back into the env it came from and replaying the
+        same actions gives the same results bit for bit, auto-resets included. A loaded env keeps its own id: its next
+        reset draws from its own random stream, so envs forked from one row are identical until their first reset.
+        Not restored: `xfrc_applied` / `qfrc_applied` (index them with the same rows), the host-side state of a custom
+        reward callback and, in the drop-in single-env mode, the host-side trajectory sampler and numpy random state.
+        Call after reset()."""
+        if self._obs is None:
+            raise RuntimeError("load_state() before the first reset(): reset first, so that envs not loaded have an observation")
+        eng = self._get_engine()
+        obs = self._obs_tensor(eng)
+        if obs.data_ptr() != eng.next_obs.data_ptr():
+            eng.next_obs.copy_(obs)
+        eng.load_state(state, index, obs_out=eng.next_obs)
+        if not self.batched:
+            self._obs = eng.next_obs[0].double().cpu().numpy()
+            return self._obs.copy()
+        self._obs = eng.next_obs.clone() if self._copy_outputs else eng.next_obs
+        return self._obs
+
+    def _obs_tensor(self, eng):
+        """The observation the env acts on next as a float32 [num_envs, obs_dim] tensor on the engine's device."""
+        if self.batched:
+            return self._obs
+        import torch
+        return torch.tensor(self._obs, dtype=torch.float32, device=eng.device).reshape(1, -1)
+
+    # ---------------------------------------------------------------------------------------------------
     # the hot path
     # ---------------------------------------------------------------------------------------------------
     def reward(self, state, action, next_state, absorbing):

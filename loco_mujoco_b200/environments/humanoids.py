@@ -313,6 +313,8 @@ class HumanoidTorque4AgesAll:
         "inverse dynamics (inverse_dynamics / create_dataset_inverse / dof_index)")
     dynamics_terms = _unavailable("the dynamics terms (dynamics_terms)")
     forward_dynamics = _unavailable("the forward dynamics (forward_dynamics)")
+    save_state = _unavailable("saved states (save_state)")
+    load_state = _unavailable("saved states (load_state)")
 
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""

@@ -21,7 +21,7 @@ def make_sharded(task_id, n_total, rank=None, world_size=None, device=None, seed
     Its `xfrc_applied` / `qfrc_applied`, `body_state` / `next_body_state`, `reference_body_state` /
     `next_reference_body_state`, `contact_wrench` and `dof_outputs`, what `inverse_dynamics(qacc)` and
     `forward_dynamics(action)` take and return and what `dynamics_terms()` returns hold the rows of this shard's envs only
-    (global env offset + i is row i)."""
+    (global env offset + i is row i). So does `save_state()`; its rows load into any shard of the same task."""
     from . import LocoEnv
     rank = dist.get_rank() if rank is None else rank
     world_size = dist.get_world_size() if world_size is None else world_size
@@ -143,7 +143,9 @@ class MixedBatch:
     So are body outputs: `envs[i].body_state` / `envs[i].next_body_state`, reference outputs:
     `envs[i].reference_body_state` / `envs[i].next_reference_body_state`, contact outputs: `envs[i].contact_wrench`, dof
     outputs: `envs[i].dof_outputs`, inverse dynamics: `envs[i].inverse_dynamics(qacc)` / `envs[i].dof_index(joint)`,
-    dynamics terms: `envs[i].dynamics_terms(...)`, and forward dynamics: `envs[i].forward_dynamics(action, ...)`.
+    dynamics terms: `envs[i].dynamics_terms(...)`, forward dynamics: `envs[i].forward_dynamics(action, ...)`, and saved
+    states: `engines[i].save_state(engines[i].next_obs)` / `engines[i].load_state(rows, index, engines[i].next_obs)` (`step`
+    drives the engines, so a member's observation to act on next is its engine's `next_obs`).
     """
 
     def __init__(self, members, device="cuda:0", seed=0, env_id_offset=0, concurrent=True, balance=True, stagger_us=40.0, **common):
