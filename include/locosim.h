@@ -214,6 +214,60 @@ int locosim_set_contact_outputs(locosim_t* h, float* d_contact);
 #define LS_DOF_DIM 3
 int locosim_set_dof_outputs(locosim_t* h, float* d_dof);
 
+/* Contact list, MuJoCo's d->contact[:d->ncon] with each contact's mj_contactForce (what a loco-mujoco user reads from
+ * env._data.contact after env.step(): support polygons, ZMP and support-margin terms, per-corner forces of box feet,
+ * penetration depth, per-pair self-collision penalties). Three caller-owned DEVICE buffers, MAXC = locosim_max_contacts(h)
+ * (the configuration's per-env contact cap, 16 in every configuration):
+ *   d_ncon    int32 [n_envs]                           the number of contacts in the list
+ *   d_con     fp32  [n_envs, MAXC, LS_CONLIST_DIM]     per contact, at the LS_CONLIST_* columns:
+ *               DIST (1)   the signed distance (negative: penetration)
+ *               POS (3)    the contact position, world frame
+ *               FRAME (9)  the contact frame's rows n, t1, t2 (world frame; n points from geom1 to geom2)
+ *               FORCE (6)  the contact-frame force f of mj_contactForce (normal, two tangents, torsion, two rolling;
+ *                          elliptic cones: the dim constraint forces; pyramidal cones: mju_decodePyramid). The components
+ *                          past dim are 0. The world-frame force is f0 n + f1 t1 + f2 t2, and it acts on geom2 (its
+ *                          negative on geom1), as in the contact outputs above.
+ *   d_con_id  int32 [n_envs, MAXC, LS_CONLIST_ID_DIM]  GEOM1, GEOM2 (the compiled model's geom indices), BODY1, BODY2
+ *                                                     (geom_bodyid: the rows of the body and contact outputs), CONDIM (dim)
+ * Rows at and past ncon are written on every step too: fp32 zeros and ids of -1, so nothing of an earlier step survives
+ * and masked reductions need no clean-up.
+ * Time window: the contact list of the control step's LAST sub-step at its last dynamics evaluation (Euler: the sub-step's
+ * only one, at its start state; RK4: its fourth stage), and that evaluation's constraint forces. This is what MuJoCo 2.3.7's
+ * mjData holds after mj_step (Euler: the mj_forward at the start of the last sub-step; RK4: mj_RungeKutta's last
+ * mj_forwardSkip, whose d->contact and d->efc_force are not restored), so the rows are what the reference's user reads
+ * after env.step(), up to fp32 and the cap. The contact outputs above are instead the MEAN over all sub-steps, summed per
+ * body. With n_substeps = 1 the two describe the same evaluation.
+ * Order: the engine's list order, the one use_foot_forces takes its "first contact" from: candidate pairs in the compiled
+ * pair table's order (primitive pairs first, then the general convex (MPR) pairs, each part in model order), and within a
+ * pair the narrow phase's order. The package's fp64 reference builds its list from the same table in the same order, so
+ * the rows match its rows one for one while nothing is dropped (tests compare them in order). MuJoCo's own broad phase may
+ * visit the pairs in another order: compare with a MuJoCo list as a set of geom pairs. Contacts the gap excludes (dist >=
+ * margin - gap), which MuJoCo keeps in d->contact without a constraint, are not in the list.
+ * Cap: contacts past MAXC, and those cut when their constraint rows would overflow the per-env row cap (DESIGN.md section
+ * 7), are not in the list and are not counted. ncon == MAXC is the only sign that contacts may have been dropped.
+ * Written by every locosim_step for every env it advances: the rows describe the step that produced d_obs (for an env that
+ * ended and was auto-reset: its terminal step; for a non-finite env ncon = 0 and empty rows). Not written by locosim_reset*,
+ * locosim_set_state or locosim_load_state.
+ * All three buffers non-NULL turns the list on; all three NULL turns it off (the state after locosim_create): nothing is
+ * written then, and no other output changes by a bit. With the buffers registered no other output changes by a bit either.
+ * Any other combination, and buffers that overlap, are refused. Register outside of stream capture.
+ * CUDA graphs: as for the contact outputs, the step kernels read the pointers from engine state on the device when they run
+ * and no kernel is added, so a step captured BEFORE the registration writes the buffers when it is replayed after it, and
+ * registering NULLs stops a captured step writing. */
+#define LS_CONLIST_DIM 19
+#define LS_CONLIST_DIST 0
+#define LS_CONLIST_POS 1
+#define LS_CONLIST_FRAME 4
+#define LS_CONLIST_FORCE 13
+#define LS_CONLIST_ID_DIM 5
+#define LS_CONLIST_GEOM1 0
+#define LS_CONLIST_GEOM2 1
+#define LS_CONLIST_BODY1 2
+#define LS_CONLIST_BODY2 3
+#define LS_CONLIST_CONDIM 4
+int locosim_max_contacts(const locosim_t* h);
+int locosim_set_contact_list_outputs(locosim_t* h, int32_t* d_ncon, float* d_con, int32_t* d_con_id);
+
 /* Replaces LocoEnv.create_dataset() (base.py:278-312 -> utils/trajectory.py:104-151) on the device: consecutive samples of
  * every trajectory of the reset table in observation layout. d_states / d_next_states fp32 [locosim_dataset_rows, obs_dim],
  * d_last fp32 [locosim_dataset_rows] (may be NULL); absorbing is all zero in the reference and is not materialised. */

@@ -1208,6 +1208,8 @@ struct locosim_handle {
   DevContact contact = {nullptr, 1};
   DevDof dof = {nullptr, 1};
   float* dof_act = nullptr;          // the dof outputs' actuator-force scratch [n_envs, nu] (c_dof_act)
+  DevConList conlist = {nullptr, 1};
+  DevConRows conrows = {nullptr, nullptr};
   DevTask dt;
   SolverOpts so;
   EngineState st;
@@ -1592,7 +1594,9 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
       cudaMemcpyToSymbol(c_refout, &h->refout, sizeof(DevRefOut), sizeof(DevRefOut) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot) != cudaSuccess ||
       cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot) != cudaSuccess ||
-      cudaMemcpyToSymbol(c_dof_act, &h->dof_act, sizeof(float*), sizeof(float*) * h->slot) != cudaSuccess) {
+      cudaMemcpyToSymbol(c_dof_act, &h->dof_act, sizeof(float*), sizeof(float*) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_conlist, &h->conlist, sizeof(DevConList), sizeof(DevConList) * h->slot) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_conrows, &h->conrows, sizeof(DevConRows), sizeof(DevConRows) * h->slot) != cudaSuccess) {
     g_create_error = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); locosim_destroy(h); return 1;
   }
   bind_task(h->dt, h->ht, h->hm.nu, h->d_tints, h->d_treals);
@@ -1829,6 +1833,33 @@ int locosim_set_dof_outputs(locosim_t* h, float* d_dof) {
   h->dof.n_substeps = h->dt.n_substeps;
   // (__constant__ tables of their own in both translation units, read when the kernels run, as for the contact outputs)
   CK(cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot));
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  return 0;
+}
+int locosim_max_contacts(const locosim_t* h) {
+  switch (h->cfg) {
+    case 0: return CfgEllEuler::MAXCON;
+    case 1: return CfgPyrEuler::MAXCON;
+    case 3: return CfgPyrEuler29::MAXCON;
+    case 4: return CfgPyrRK4_31::MAXCON;
+    case 5: return CfgPyrEuler31::MAXCON;
+    default: return CfgPyrRK4::MAXCON;
+  }
+}
+int locosim_set_contact_list_outputs(locosim_t* h, int32_t* d_ncon, float* d_con, int32_t* d_con_id) {
+  const int on = (d_ncon != nullptr) + (d_con != nullptr) + (d_con_id != nullptr);
+  if (on != 0 && on != 3) { h->err = "contact list: pass all three buffers or none"; return 1; }
+  const size_t n = (size_t)h->n_envs, C = (size_t)locosim_max_contacts(h);
+  const void* const buf[3] = {d_ncon, d_con, d_con_id};
+  const size_t bytes[3] = {n * 4, n * C * LS_CONLIST_DIM * 4, n * C * LS_CONLIST_ID_DIM * 4};
+  if (buffers_overlap(buf, bytes, 3)) { h->err = "contact list buffers overlap"; return 1; }
+  CK(cudaSetDevice(h->device));
+  h->conlist.ncon = d_ncon; h->conrows.con = d_con; h->conrows.id = d_con_id;
+  h->conlist.n_substeps = h->dt.n_substeps;
+  // (__constant__ tables of their own in both translation units, read when the kernels run, as for the contact outputs; the
+  // rows first, so that a kernel never sees the count pointer without them)
+  CK(cudaMemcpyToSymbol(c_conrows, &h->conrows, sizeof(DevConRows), sizeof(DevConRows) * h->slot));
+  CK(cudaMemcpyToSymbol(c_conlist, &h->conlist, sizeof(DevConList), sizeof(DevConList) * h->slot));
   if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
   return 0;
 }

@@ -45,6 +45,8 @@ int locosim_configs31_sync_model(Handle31* h) {
   CK(cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot));
   CK(cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot));
   CK(cudaMemcpyToSymbol(c_dof_act, &h->dof_act, sizeof(float*), sizeof(float*) * h->slot));
+  CK(cudaMemcpyToSymbol(c_conrows, &h->conrows, sizeof(DevConRows), sizeof(DevConRows) * h->slot));
+  CK(cudaMemcpyToSymbol(c_conlist, &h->conlist, sizeof(DevConList), sizeof(DevConList) * h->slot));
   return 0;
 }
 

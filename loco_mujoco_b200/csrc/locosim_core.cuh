@@ -153,6 +153,19 @@ struct DevDof {
   int n_substeps;
 };
 
+// contact list of a handle (locosim_set_contact_list_outputs): caller-owned [N] contact counts, [N, MAXCON, LS_CONLIST_DIM]
+// rows (dist, pos, frame, contact-frame force) and [N, MAXCON, LS_CONLIST_ID_DIM] ids (geom1, geom2, body1, body2, dim),
+// row EnvS::env, the contacts of the control step's last sub-step; NULL = not written. Two tables of DevDof's 16-byte
+// layout: physics_substeps tests `ncon`, and a 32-byte stride grew the CfgPyrRK4 step kernel's stack frame by 16 bytes.
+struct DevConList {
+  int* ncon;
+  int n_substeps;
+};
+struct DevConRows {
+  float* con;
+  int* id;
+};
+
 struct DevTask {
   int obs_dim, n_done, reward_type, n_substeps, n_traj, traj_len, n_goal, recenter0, recenter1, ri[4], use_absorbing;
   int n_grf;                      // foot-force groups (use_foot_forces), 0 = off
@@ -174,6 +187,8 @@ static DevBodyOut c_bodyout[LS_MAX_SLOTS];
 static DevContact c_contact[LS_MAX_SLOTS];
 static DevDof c_dof[LS_MAX_SLOTS];
 static float* c_dof_act[LS_MAX_SLOTS];
+static DevConList c_conlist[LS_MAX_SLOTS];
+static DevConRows c_conrows[LS_MAX_SLOTS];
 static int c_debug = 0;
 #else
 __constant__ DevModel c_models[LS_MAX_SLOTS];
@@ -189,6 +204,8 @@ __constant__ DevDof c_dof[LS_MAX_SLOTS];          // (a table of its own, like c
 // registered (the actuator force is folded into qfrc_smooth, and the Euler state it was evaluated at is gone after the
 // integrator), read by dof_outputs
 __constant__ float* c_dof_act[LS_MAX_SLOTS];
+__constant__ DevConList c_conlist[LS_MAX_SLOTS];  // (a table of its own, like c_contact)
+__constant__ DevConRows c_conrows[LS_MAX_SLOTS];  // (likewise)
 __device__ unsigned long long g_dbg[8];      // (LOCOSIM_DEBUG & 8) MPR statistics: calls, support pairs, hits, cap exits
 #endif
 
@@ -246,9 +263,9 @@ struct alignas(16) EnvS {
   float xpos[NB][3], xquat[NB][4], xmat[NB][9];
   float gxpos[NG][3];
   float com[3];
-  int substep;             // contact / dof outputs: index within the control step of the next sub-step (-1: a warp that
-                           // shadows another env, which writes no outputs); set by the kernels, advanced by contact_wrench
-                           // (or by dof_outputs when only those are registered)
+  int substep;             // contact / dof outputs, contact list: index within the control step of the next sub-step (-1: a
+                           // warp that shadows another env, which writes no outputs); set by the kernels, advanced by
+                           // contact_wrench (or by dof_outputs when it is not registered, or by contact_list when neither is)
   float cdof[NV][6];
   float M[NV][NVP], H[NV][NVP];                              // H: chol(M) during smooth_forces, then the Newton Hessian factor
   // contacts
@@ -3223,10 +3240,59 @@ LS_FN void dof_outputs(const int ms, EnvS<C>& e) {
   }
 }
 
+// contact list (locosim_set_contact_list_outputs): at the control step's last sub-step (k == n_sub - 1) the contact list of
+// its last forward evaluation, in list order, into the env's rows of the caller's buffers: lane ci writes row ci, contacts
+// below ncon from EnvS (the frame, position and dist of fill_contact; f of contact_frame_force, as mj_contactForce), every
+// other row zeros and ids -1; a non-finite env (the epilogue's test on the same state) gets ncon = 0. Earlier sub-steps
+// write nothing. Runs before dof_outputs and contact_wrench and advances EnvS::substep only when neither will.
+template <class C>
+LS_FN void contact_list(const int ms, EnvS<C>& e) {
+  static_assert(C::MAXCON <= 32, "contact_list: one lane per contact");
+  const int k = e.substep;
+  if (k < 0) return;
+  const DevConList& cl = c_conlist[ms];
+  if (k == cl.n_substeps - 1) {
+    const DevModel& m = c_models[ms];
+    bool bad = false;
+    PAR_FOR(i, m.nv) bad |= !(isfinite(e.qpos[i]) && isfinite(e.qvel[i]));
+#ifndef LS_EMULATE
+    bad = __any_sync(0xffffffffu, bad);
+#endif
+    const int ncon = bad ? 0 : e.ncon;
+    float* rows = c_conrows[ms].con + (size_t)e.env * C::MAXCON * LS_CONLIST_DIM;
+    int* ids = c_conrows[ms].id + (size_t)e.env * C::MAXCON * LS_CONLIST_ID_DIM;
+    PAR_FOR(ci, C::MAXCON) {
+      float* r = rows + ci * LS_CONLIST_DIM;
+      int* d = ids + ci * LS_CONLIST_ID_DIM;
+      if (ci < ncon) {
+        float f[6];
+        contact_frame_force(e, ci, f);
+        const int g1 = e.con_g1[ci], g2 = e.con_g2[ci];
+        r[LS_CONLIST_DIST] = e.con_dist[ci];
+        for (int c = 0; c < 3; c++) r[LS_CONLIST_POS + c] = e.con_pos[ci][c];
+        for (int c = 0; c < 9; c++) r[LS_CONLIST_FRAME + c] = e.con_frame[ci][c];
+        for (int c = 0; c < 6; c++) r[LS_CONLIST_FORCE + c] = f[c];
+        d[LS_CONLIST_GEOM1] = g1; d[LS_CONLIST_GEOM2] = g2;
+        d[LS_CONLIST_BODY1] = m.geom_bodyid[g1]; d[LS_CONLIST_BODY2] = m.geom_bodyid[g2];
+        d[LS_CONLIST_CONDIM] = e.con_dim[ci];
+      } else {
+        for (int c = 0; c < LS_CONLIST_DIM; c++) r[c] = 0.0f;
+        for (int c = 0; c < LS_CONLIST_ID_DIM; c++) d[c] = -1;
+      }
+    }
+    LANE0 cl.ncon[e.env] = ncon;
+    SYNC();
+  }
+  if (!c_dof[ms].out && !c_contact[ms].wrench) {
+    LANE0 e.substep = k + 1;
+    SYNC();
+  }
+}
+
 // use_foot_forces (base.py:623-631,656-679 -> mushroom _get_collision_force -> mj_contactForce): per foot group the
 // contact-frame force (normal, tangent 1, tangent 2) of the FIRST contact between the floor and a geom of the group, in
 // contact-list order, from the constraint forces of the sub-step's (last) forward evaluation; summed over sub-steps. Then
-// the contact outputs of the sub-step, while registered.
+// the contact list, the dof outputs and the contact outputs of the sub-step, each while registered.
 template <class C>
 LS_FN void contact_forces(const int ms, EnvS<C>& e, const int* grf_group, int n_grf) {
   const int nunit = e.nunit, ncon = e.ncon;
@@ -3257,6 +3323,7 @@ LS_FN void contact_forces(const int ms, EnvS<C>& e, const int* grf_group, int n_
     }
   }
   SYNC();
+  if (c_conlist[ms].ncon) contact_list(ms, e);
   if (c_dof[ms].out) dof_outputs(ms, e);
   if (c_contact[ms].wrench) contact_wrench(ms, e);
 }
@@ -3269,9 +3336,9 @@ LS_FN void physics_substeps(const int ms, EnvS<C>& e, const SolverOpts so, int n
     forward(ms, e, so);
     PH_T0(t);
     if constexpr (C::RK4 == 1) rk4_step(ms, e, so); else euler_step(ms, e);
-    // (the contact and dof outputs are written from contact_forces' call rather than calls of their own: another call site
-    //  here changes the step kernels' register allocation and spills whether or not anything is registered)
-    if (n_grf > 0 || c_contact[ms].wrench || c_dof[ms].out) contact_forces(ms, e, grf_group, n_grf);
+    // (the contact and dof outputs and the contact list are written from contact_forces' call rather than calls of their own:
+    //  another call site here changes the step kernels' register allocation and spills whether or not anything is registered)
+    if (n_grf > 0 || c_contact[ms].wrench || c_dof[ms].out || c_conlist[ms].ncon) contact_forces(ms, e, grf_group, n_grf);
     PH_LAP(PH_INTEGRATOR, t);
     PH_LAP(PH_SUBSTEP, t_sub);
     PH_CNT(PH_SUBSTEPS, 1);

@@ -14,6 +14,8 @@ struct EmuBase {
   DevApplied ap = {nullptr, nullptr};
   DevContact cw = {nullptr, 1};
   DevDof dof = {nullptr, 1};
+  DevConList cl = {nullptr, 1};
+  DevConRows cr = {nullptr, nullptr};
   std::vector<float> act;            // the dof outputs' actuator-force scratch (row 0 of the engine's [N, nu])
   SolverOpts so;
   std::vector<int> grf_group; int n_grf = 0;
@@ -34,6 +36,7 @@ struct EmuBase {
   virtual void inv(const double* qacc, float* out) = 0;
   virtual void dyn(const DynOut& o) = 0;
   virtual void fwd_out(const double* ctrl, const FwdOut& o) = 0;
+  virtual int max_contacts() = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -46,6 +49,7 @@ struct EmuT : EmuBase {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
     c_models[0] = m; c_applied[0] = ap; c_contact[0] = cw; c_contact[0].n_substeps = nsub;
     c_dof[0] = dof; c_dof[0].n_substeps = nsub; c_dof_act[0] = dof.out ? act.data() : nullptr;
+    c_conlist[0] = cl; c_conlist[0].n_substeps = nsub; c_conrows[0] = cr;
     e.substep = 0;
     physics_substeps(0, e, so, nsub, grf_group.data(), n_grf);
   }
@@ -117,6 +121,7 @@ struct EmuT : EmuBase {
     init_workspace(0, e);
     forward_dynamics(0, e, so, o);
   }
+  int max_contacts() override { return C::MAXCON; }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
 
@@ -200,6 +205,14 @@ void emu_set_dof(EmuBase* s, float* out) {
   s->act.assign(s->m.nu > 0 ? s->m.nu : 1, 0.0f);
   s->dof.out = out;
 }
+// contact list of the emulated env (locosim_set_contact_list_outputs; row 0 of the engine's layout: int32 [1], fp32
+// [MAXCON, LS_CONLIST_DIM], int32 [MAXCON, LS_CONLIST_ID_DIM], all three or all NULL): every later emu_step(ctrl, nsub) runs
+// as one control step of nsub sub-steps and leaves the list of its last sub-step there
+void emu_set_contact_list(EmuBase* s, int* ncon, float* con, int* id) {
+  s->cl.ncon = ncon; s->cr.con = con; s->cr.id = id;
+}
+// the configuration's per-env contact cap (locosim_max_contacts)
+int emu_max_contacts(EmuBase* s) { return s->max_contacts(); }
 long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, g_obb_pass}; return v[k]; }
 // the diagnostic switches of the emulated engine (LOCOSIM_DEBUG; e.g. 32: no capsule-hull test)
 void emu_set_debug(int v) { c_debug = v; }

@@ -103,6 +103,10 @@ def load_library():
     lib.locosim_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.locosim_state_words.restype = ip
     lib.locosim_state_words.argtypes = [vp]
+    lib.locosim_max_contacts.restype = ip
+    lib.locosim_max_contacts.argtypes = [vp]
+    lib.locosim_set_contact_list_outputs.restype = ip
+    lib.locosim_set_contact_list_outputs.argtypes = [vp, vp, vp, vp]
     lib.locosim_save_state.restype = ip
     lib.locosim_save_state.argtypes = [vp, vp, vp, vp]
     lib.locosim_load_state.restype = ip
@@ -122,7 +126,8 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_set_body_outputs", "locosim_set_contact_outputs", "locosim_set_dof_outputs",
                     "locosim_set_reference_outputs", "locosim_create_dataset_bodies", "locosim_inverse",
                     "locosim_create_dataset_inverse", "locosim_dynamics_terms", "locosim_forward", "locosim_state_words",
-                    "locosim_save_state", "locosim_load_state"]
+                    "locosim_save_state", "locosim_load_state", "locosim_max_contacts",
+                    "locosim_set_contact_list_outputs"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -136,6 +141,12 @@ COM_DIM = 4
 # values per body row of the forward dynamics' body accelerations (include/locosim.h LS_BODY_ACC_DIM): angular acceleration
 # (3), linear acceleration of the body-frame origin minus gravity (3), world frame
 BODY_ACC_DIM = 6
+# values per contact row of the contact list (include/locosim.h LS_CONLIST_DIM / LS_CONLIST_ID_DIM) and their columns
+# (LS_CONLIST_*): dist (1), pos (3), frame rows n, t1, t2 (9), contact-frame force (6); geom1, geom2, body1, body2, dim
+CONLIST_DIM = 19
+CONLIST_COLUMNS = dict(dist=(0, 1), pos=(1, 3), frame=(4, 9), force=(13, 6))
+CONLIST_ID_DIM = 5
+CONLIST_ID_COLUMNS = dict(geom=(0, 2), body=(2, 2), dim=(4, 1))
 
 
 
@@ -219,6 +230,7 @@ class CudaEngine:
         self._body_out = (None, None)     # the registered body-output tensors (likewise)
         self._contact_out = None          # the registered contact-output tensor (likewise)
         self._dof_out = None              # the registered dof-output tensor (likewise)
+        self._conlist_out = (None, None, None)   # the registered contact-list tensors (likewise)
         self._ref_out = (None, None)      # the registered reference-output tensors (likewise)
         # obs / reward / done of a step live in ONE device allocation (three views), so that a consumer on the host can
         # fetch the whole step result with a single D2H copy of `packed_out`
@@ -229,6 +241,7 @@ class CudaEngine:
         self.launches = 0
         self.kernels_per_step = self.lib.locosim_kernels_per_step(h)
         self.state_words = self.lib.locosim_state_words(h)
+        self.max_contacts = self.lib.locosim_max_contacts(h)
 
     def views_of(self, packed):
         """(obs [N, D] f32, reward [N] f32, done [N] u8) views of a buffer laid out like `packed_out`."""
@@ -398,6 +411,26 @@ class CudaEngine:
             self._check_tensor(dof, "dof", (self.n_envs, self.nq, DOF_DIM))
         self._check(self.lib.locosim_set_dof_outputs(self.h, _ptr(dof)))
         self._dof_out = dof
+
+    def set_contact_list_outputs(self, ncon=None, con=None, con_id=None):
+        """Register the contact list of include/locosim.h (MuJoCo's d.contact with each contact's mj_contactForce): `ncon`
+        int32 cuda [n_envs], `con` float32 cuda [n_envs, max_contacts, CONLIST_DIM] and `con_id` int32 cuda [n_envs,
+        max_contacts, CONLIST_ID_DIM], all three, or none to turn the feature off. Every step writes the contacts of its
+        last sub-step in list order (CONLIST_COLUMNS / CONLIST_ID_COLUMNS), zeros and ids of -1 in the rows past ncon, and
+        ncon = 0 for a non-finite env. reset(), set_state() and load_state() leave them alone. The engine keeps references
+        to them. Register outside of CUDA-graph capture; a step captured earlier writes the buffers registered when it is
+        replayed."""
+        bufs = (ncon, con, con_id)
+        if any(x is None for x in bufs) and any(x is not None for x in bufs):
+            raise ValueError("ncon, con and con_id must be given together (or none of them)")
+        n, C = self.n_envs, self.max_contacts
+        spans = (("ncon", ncon, (n,)), ("con", con, (n, C, CONLIST_DIM)), ("con_id", con_id, (n, C, CONLIST_ID_DIM)))
+        if ncon is not None:
+            for (name, x, shape), dtype in zip(spans, ("int32", "float32", "int32")):
+                self._check_tensor(x, name, shape, dtype)
+            self._check_disjoint(spans)
+        self._check(self.lib.locosim_set_contact_list_outputs(self.h, _ptr(ncon), _ptr(con), _ptr(con_id)))
+        self._conlist_out = bufs
 
     def episode_stats(self):
         """(length int32, return float32, last_length, last_return), each [n_envs]: the running episode's control steps and

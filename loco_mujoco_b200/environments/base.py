@@ -17,6 +17,7 @@ All physics runs in the CUDA engine (loco_mujoco_b200/csrc); there is no CPU pat
 """
 import os
 import warnings
+from collections import namedtuple
 from copy import deepcopy
 from itertools import product
 
@@ -28,6 +29,9 @@ from ..task import (TaskSpec, OBS_QPOS, OBS_QVEL, OBS_GOAL, OBS_GRF, OBS_PARAM, 
                     REWARD_POS, REWARD_TRACKING)
 from ..trajectory import Trajectory
 from ..utils.reward import NoReward, CustomReward, TargetVelocityReward, PosReward
+
+# LocoEnv.contacts: torch views of the engine's contact-list buffers (include/locosim.h locosim_set_contact_list_outputs)
+ContactList = namedtuple("ContactList", "ncon dist pos frame force geom body dim")
 
 
 class ObservationType:
@@ -245,6 +249,8 @@ class LocoEnv:
         self._contact_wrench = None
         # dof outputs (dof_outputs below): allocated and registered with the engine on first access
         self._dof_outputs = None
+        # contact list (contacts below): (ncon, con, con_id) allocated and registered with the engine on first access
+        self._contact_list = None
         # reference outputs (reference_body_state / next_reference_body_state below): likewise
         self._reference_body_state = None
         self._next_reference_body_state = None
@@ -446,6 +452,8 @@ class LocoEnv:
                 self._engine.set_contact_outputs(self._contact_wrench)
             if self._dof_outputs is not None:
                 self._engine.set_dof_outputs(self._dof_outputs)
+            if self._contact_list is not None:
+                self._engine.set_contact_list_outputs(*self._contact_list[:3])
             if self._reference_body_state is not None:
                 self._engine.set_reference_outputs(self._reference_body_state, self._next_reference_body_state)
         return self._engine
@@ -571,6 +579,59 @@ class LocoEnv:
             eng.set_dof_outputs(t)
             self._dof_outputs = t
         return self._dof_outputs
+
+    # ---------------------------------------------------------------------------------------------------
+    # contact list (MuJoCo's d.contact and mj_contactForce, include/locosim.h locosim_set_contact_list_outputs)
+    # ---------------------------------------------------------------------------------------------------
+    @property
+    def contacts(self):
+        """The contact list of each env, rewritten by every step: a ContactList of torch views on the env's device, C =
+        the engine's per-env contact cap (16):
+            ncon   int32 [num_envs]           contacts in the list
+            dist   float32 [num_envs, C]      signed distance (negative: penetration)
+            pos    float32 [num_envs, C, 3]   contact position, world frame
+            frame  float32 [num_envs, C, 3, 3] rows n, t1, t2 of the contact frame (n points from geom1 to geom2)
+            force  float32 [num_envs, C, 6]   mj_contactForce's contact-frame force (normal, tangents, torsion, rolling;
+                                              zeros past dim); it acts on geom2, its negative on geom1
+            geom   int32 [num_envs, C, 2]     geom1, geom2: indices of the compiled model (`geom_index`, `geom_names`)
+            body   int32 [num_envs, C, 2]     their bodies (`body_index`, the rows of `contact_wrench` and `body_state`)
+            dim    int32 [num_envs, C]        condim of the contact
+        The list is the one MuJoCo's mjData holds after mj_step, the contacts and forces of the step's LAST sub-step (its
+        last dynamics evaluation), in the engine's list order (the compiled pair table's, as MuJoCo's); `contact_wrench` is
+        instead the mean over all sub-steps, summed per body. Contacts past the cap are dropped: ncon == C is the only sign.
+        Rows at and past ncon hold zeros and ids of -1. It describes the step that produced the observation: for an env
+        that ended, its terminal step; for an env whose state became non-finite, ncon = 0. reset(), set_state() and
+        load_state() do not write it. Allocated and registered on first access: an env that never touches it computes
+        nothing extra. A step captured in a CUDA graph before the first access writes it from the next replay on."""
+        if self._contact_list is None:
+            import torch
+            from ..engine import CONLIST_DIM, CONLIST_ID_DIM, CONLIST_COLUMNS as F, CONLIST_ID_COLUMNS as I
+            eng = self._get_engine()
+            n, C, dev = self.num_envs, eng.max_contacts, eng.device
+            ncon = torch.zeros((n,), dtype=torch.int32, device=dev)
+            con = torch.zeros((n, C, CONLIST_DIM), dtype=torch.float32, device=dev)
+            con_id = torch.full((n, C, CONLIST_ID_DIM), -1, dtype=torch.int32, device=dev)
+            eng.set_contact_list_outputs(ncon, con, con_id)
+            col = lambda t, c: t[:, :, c[0]:c[0] + c[1]]      # noqa: E731
+            self._contact_list = (ncon, con, con_id, ContactList(
+                ncon=ncon, dist=con[:, :, F["dist"][0]], pos=col(con, F["pos"]),
+                frame=col(con, F["frame"]).unflatten(-1, (3, 3)), force=col(con, F["force"]), geom=col(con_id, I["geom"]),
+                body=col(con_id, I["body"]), dim=con_id[:, :, I["dim"][0]]))
+        return self._contact_list[3]
+
+    @property
+    def geom_names(self):
+        """Names of the compiled model's geoms, by index (the ids of `contacts.geom`; None for an unnamed geom). Geoms that
+        take part in no collision (contype and conaffinity 0: visual only) are dropped by the compiler and are not there."""
+        return list(self._model.geom_names)
+
+    def geom_index(self, name):
+        """Index of geom `name` in the compiled model (as `contacts.geom` holds it). ValueError for an unknown name and for a
+        visual-only geom, which the compiler drops."""
+        if name is not None and name in self._model.geom_names:
+            return self._model.geom_names.index(name)
+        raise ValueError("unknown geom %r (visual-only geoms, contype = conaffinity = 0, are not compiled; geoms of the "
+                         "compiled model: %s)" % (name, ", ".join(str(g) for g in self._model.geom_names)))
 
     # ---------------------------------------------------------------------------------------------------
     # reference outputs (the mocap clip's body outputs, include/locosim.h locosim_set_reference_outputs)

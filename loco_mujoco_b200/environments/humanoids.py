@@ -306,6 +306,8 @@ class HumanoidTorque4AgesAll:
     body_state = next_body_state = property(_unavailable("body outputs (body_state / next_body_state)"))
     contact_wrench = property(_unavailable("contact outputs (contact_wrench)"))
     dof_outputs = property(_unavailable("dof outputs (dof_outputs)"))
+    geom_index = _unavailable("contact lists (contacts / geom_index / geom_names)")
+    contacts = geom_names = property(geom_index)
     create_dataset_bodies = _unavailable("reference outputs (reference_body_state / next_reference_body_state / "
                                          "create_dataset_bodies)")
     reference_body_state = next_reference_body_state = property(create_dataset_bodies)

@@ -19,7 +19,7 @@ def shard_range(n_total, world_size, rank):
 def make_sharded(task_id, n_total, rank=None, world_size=None, device=None, seed=0, **kwargs):
     """LocoEnv for this rank's shard; `env_id_offset` keeps every env's random stream identical to the 1-GPU run.
     Its `xfrc_applied` / `qfrc_applied`, `body_state` / `next_body_state`, `reference_body_state` /
-    `next_reference_body_state`, `contact_wrench` and `dof_outputs`, what `inverse_dynamics(qacc)` and
+    `next_reference_body_state`, `contact_wrench`, `dof_outputs` and `contacts`, what `inverse_dynamics(qacc)` and
     `forward_dynamics(action)` take and return and what `dynamics_terms()` returns hold the rows of this shard's envs only
     (global env offset + i is row i). So does `save_state()`; its rows load into any shard of the same task."""
     from . import LocoEnv
@@ -142,7 +142,7 @@ class MixedBatch:
     Applied forces are per member: `envs[i].xfrc_applied` / `envs[i].qfrc_applied` / `envs[i].body_index(name)`.
     So are body outputs: `envs[i].body_state` / `envs[i].next_body_state`, reference outputs:
     `envs[i].reference_body_state` / `envs[i].next_reference_body_state`, contact outputs: `envs[i].contact_wrench`, dof
-    outputs: `envs[i].dof_outputs`, inverse dynamics: `envs[i].inverse_dynamics(qacc)` / `envs[i].dof_index(joint)`,
+    outputs: `envs[i].dof_outputs`, the contact list: `envs[i].contacts`, inverse dynamics: `envs[i].inverse_dynamics(qacc)` / `envs[i].dof_index(joint)`,
     dynamics terms: `envs[i].dynamics_terms(...)`, forward dynamics: `envs[i].forward_dynamics(action, ...)`, and saved
     states: `engines[i].save_state(engines[i].next_obs)` / `engines[i].load_state(rows, index, engines[i].next_obs)` (`step`
     drives the engines, so a member's observation to act on next is its engine's `next_obs`).
