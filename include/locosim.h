@@ -455,6 +455,48 @@ int locosim_state_words(const locosim_t* h);
 int locosim_save_state(locosim_t* h, const float* d_obs, int32_t* d_state, void* stream);
 int locosim_load_state(locosim_t* h, const int32_t* d_state, int n_rows, const int32_t* d_row, float* d_obs, void* stream);
 
+/* Ray casting against every env's geoms, MuJoCo 2.3.7's mj_ray for a batch of rays (what a loco-mujoco user builds
+ * rangefinders, height scans, distance-to-obstacle terms and depth or segmentation cameras from). Every env is taken at its
+ * stored state (what locosim_get_state returns, the state of info["next_obs"]) with its current parameter-pool row, and the
+ * kinematics of the body outputs.
+ *   d_pnt, d_vec  fp32 [n_rays, 3] shared by every env, or [n_envs, n_rays, 3] with LS_RAY_PER_ENV: the ray pnt + x vec, in
+ *                 the query frame:
+ *                   LS_RAY_WORLD    world coordinates (frame_body is not read, but must be a body index)
+ *                   LS_RAY_BODY     the frame (xpos, xquat) of body frame_body, as in the body outputs
+ *                   LS_RAY_HEADING  at xpos of frame_body, rotated about the world z axis by the yaw of the body's x axis (a
+ *                                   heading frame: height scans that turn with the robot but stay level)
+ *                   LS_RAY_TRACK    at xpos of frame_body with the world's axes (a tracking camera)
+ *   d_dist        fp32 [n_envs, n_rays]: the smallest x >= 0 for which pnt + x vec lies on a selected geom's surface, in units
+ *                 of |vec| (a unit vec gives metres), or -1 when nothing is hit, and for a zero vec
+ *   d_geom        int32 [n_envs, n_rays]: that geom's index in the compiled model (the ids of the contact list), or -1
+ *   d_normal      fp32 [n_envs, n_rays, 3] or NULL: the outward unit normal of the surface at the hit, world frame; zeros when
+ *                 nothing is hit. (MuJoCo 2.3.7's mj_ray has no normal: this one is defined here; shading uses it.)
+ *   exclude_body  MuJoCo's bodyexclude: the geoms of this body are skipped; -1: none
+ *   flags         LS_RAY_STATIC: geoms on bodies welded to the world (no joint on their path to it: MuJoCo's flg_static,
+ *                 the floor); LS_RAY_DYNAMIC: every other geom (the robot's); both: every geom
+ * Geometry: every geom the engine collides with. Plane, sphere, capsule, ellipsoid, cylinder and box follow MuJoCo 2.3.7's
+ * engine_ray.c: a plane is hit from its +z side only, and only within size[0] x size[1] where those are non-zero; a ray that
+ * starts inside a solid primitive reports where it leaves it (the smallest non-negative root). A mesh geom is cast against
+ * the convex hull of its compiled vertices, the shape the engine collides with (MuJoCo casts against the mesh's own
+ * triangles: a non-convex mesh differs in its concave parts); a ray that starts inside a hull reports where it leaves it.
+ * Geom groups and rgba are not part of the compiled model, so they select nothing (MuJoCo's geomgroup filter and its
+ * skipping of invisible geoms have no counterpart), and visual-only geoms are not there to be hit.
+ * A non-finite qpos or qvel of an env gives that env -1 and zeros. NULL d_pnt, d_vec, d_dist or d_geom, n_rays < 1, an
+ * unknown frame or flag bit, frame_body or exclude_body out of range, outputs that overlap each other or the inputs, and a
+ * launch grid the device cannot take (more than 65535 * 128 rays per env) are refused. The call changes nothing: state, warm
+ * start, counters, cursors, random streams, episode statistics and every registered output stay as they were, so a step after
+ * it is bit-identical to the same step without it. Stream-ordered, no host synchronisation, no allocation: it can be
+ * captured in a CUDA graph (a replay reads the rays and the state as they are then). */
+#define LS_RAY_WORLD 0
+#define LS_RAY_BODY 1
+#define LS_RAY_HEADING 2
+#define LS_RAY_TRACK 3
+#define LS_RAY_STATIC 1
+#define LS_RAY_DYNAMIC 2
+#define LS_RAY_PER_ENV 4
+int locosim_ray(locosim_t* h, const float* d_pnt, const float* d_vec, int n_rays, int frame, int frame_body,
+                int exclude_body, int flags, float* d_dist, int32_t* d_geom, float* d_normal, void* stream);
+
 /* Per-episode goal features (UnitreeA1: cos / sin of the goal direction and the goal speed, GoalDirectionVelocity set in
  * setup() unitreeA1.py:287-291); normally loaded from the reset table, settable for reset(obs=...) (base.py:217-218,633-654).
  * d_goal fp32 [n_envs, 4]. */

@@ -1153,6 +1153,60 @@ __global__ void __launch_bounds__(32) forward_kernel(int ms, EngineState st, Dev
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// Ray casting (locosim_ray). Block (env, chunk) casts rays [chunk * LS_RAY_BLOCK, +LS_RAY_BLOCK) of env `env`: warp 0 runs
+// kinematics() on the block's EnvS at the env's stored state and pool row, the block stages every geom's world frame into
+// a RayGeom table behind the EnvS, then each thread casts one ray against the whole table (ray_geoms). The engine's state
+// is only read. Instantiated in locosim_ray.cu only: the step kernels' translation units compile none of this code.
+// ----------------------------------------------------------------------------------------------------------
+#define LS_RAY_BLOCK 128
+struct RayArgs {
+  const float *pnt, *vec;          // [n_rays, 3] or, with LS_RAY_PER_ENV, [n_envs, n_rays, 3]
+  float* dist;                     // [n_envs, n_rays]
+  int* geom;                       // [n_envs, n_rays]
+  float* normal;                   // [n_envs, n_rays, 3] or NULL
+  int n_rays, frame, frame_body, exclude, flags;
+};
+template <class C>
+__global__ void __launch_bounds__(LS_RAY_BLOCK) ray_kernel(int ms, EngineState st, RayArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  EnvS<C>& e = *reinterpret_cast<EnvS<C>*>(smem_raw);
+  RayGeom* G = reinterpret_cast<RayGeom*>(smem_raw + sizeof(EnvS<C>));
+  __shared__ int bad;
+  const DevModel& m = c_models[ms];
+  const int r = blockIdx.x, nv = m.nv, ng = m.ng;
+  if (threadIdx.x < 32) {
+    if (threadIdx.x == 0) e.prm = st.pool + (size_t)st.dr_row[r] * m.pool_P;
+    for (int i = threadIdx.x; i < nv; i += 32) {
+      e.qpos[i] = st.qpos[(size_t)r * nv + i];
+      e.qvel[i] = st.qvel[(size_t)r * nv + i];
+    }
+    __syncwarp();
+    const bool nf = nonfinite_state(e, nv);
+    if (!nf) kinematics(ms, e);
+    if (threadIdx.x == 0) bad = nf;
+  }
+  __syncthreads();
+  if (!bad)
+    for (int g = threadIdx.x; g < ng; g += blockDim.x) ray_stage_geom(ms, e, g, G[g]);
+  __syncthreads();
+  const int k = blockIdx.y * blockDim.x + threadIdx.x;
+  if (k >= a.n_rays) return;
+  const size_t o = (size_t)r * a.n_rays + k, src = 3 * ((a.flags & LS_RAY_PER_ENV) ? o : (size_t)k);
+  float dist = -1, nrm[3] = {0, 0, 0};
+  int geom = -1;
+  if (!bad) {
+    const float pnt[3] = {__ldg(a.pnt + src), __ldg(a.pnt + src + 1), __ldg(a.pnt + src + 2)};
+    const float vec[3] = {__ldg(a.vec + src), __ldg(a.vec + src + 1), __ldg(a.vec + src + 2)};
+    float p[3], v[3];
+    ray_to_world(e, a.frame, a.frame_body, pnt, vec, p, v);
+    dist = ray_geoms(G, ng, p, v, a.exclude, a.flags, &geom, nrm);
+  }
+  a.dist[o] = dist;
+  a.geom[o] = geom;
+  if (a.normal) for (int c = 0; c < 3; c++) a.normal[3 * o + c] = nrm[c];
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // Regrouping: the warps of a block run the solver in lock-step, so a block is as slow as its hardest env. Solver effort
 // is strongly correlated from one control step to the next (lag-1 correlation of the per-step Newton iteration count
 // ~0.6), so before every step the envs are bucketed by the iteration count of their previous step (counting sort,
@@ -1306,6 +1360,16 @@ static int launch_forward(locosim_handle* h, const float* action, const FwdOut& 
   so.sync_phases = 0;
   forward_kernel<RoundLoop<C>><<<h->n_envs, 32, sizeof(EnvS<C>), s>>>(h->slot, h->st, h->dt, (const int*)h->d_stage, so,
                                                                        action, o);
+  CK(cudaGetLastError());
+  return 0;
+}
+// ray_kernel with inverse_kernel's configuration type (locosim_ray.cu); the caller has checked the grid's y extent
+template <class C>
+static int launch_ray(locosim_handle* h, const RayArgs& a, cudaStream_t s) {
+  constexpr size_t smem = sizeof(EnvS<C>) + sizeof(RayGeom) * C::NG;
+  static_assert(smem <= 48 * 1024, "ray_kernel: one EnvS and the geom table per block within the default shared-memory limit");
+  const dim3 grid((unsigned)h->n_envs, (unsigned)((a.n_rays + LS_RAY_BLOCK - 1) / LS_RAY_BLOCK));
+  ray_kernel<RoundLoop<C>><<<grid, LS_RAY_BLOCK, smem, s>>>(h->slot, h->st, a);
   CK(cudaGetLastError());
   return 0;
 }
@@ -1504,6 +1568,10 @@ extern "C" int locosim_configs31_dataset_inverse(locosim_handle* h, float* qfrc,
 extern "C" int locosim_configs31_dynamics(locosim_handle* h, const DynOut* o, cudaStream_t s) __attribute__((weak));
 extern "C" int locosim_configs31_forward(locosim_handle* h, const float* action, const FwdOut* o, cudaStream_t s)
     __attribute__((weak));
+// The ray kernels of all six configurations are compiled in a third translation unit, locosim_ray.cu, with its own
+// __constant__ model slots (written at create and after a parameter-pool upload). Weak like the 31-dof entry points.
+extern "C" int locosim_ray_sync_model(locosim_handle* h) __attribute__((weak));
+extern "C" int locosim_ray_launch(locosim_handle* h, const RayArgs* a, cudaStream_t s) __attribute__((weak));
 
 // body_kernel outside a step, for the envs of `mask` (NULL = all), the parts (see body_kernel) that are registered:
 // d_next_body (1) after locosim_reset* and locosim_set_state; the reference keys (2) and d_next_ref (4) after locosim_reset*,
@@ -1617,6 +1685,7 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
       break;
     default: rc = setup_cfg<CfgPyrRK4>(h); break;
   }
+  if (!rc && locosim_ray_sync_model) rc = locosim_ray_sync_model(h);
   if (rc) { g_create_error = h->err; locosim_destroy(h); return 1; }
   *out = h;
   return 0;
@@ -1811,6 +1880,29 @@ int locosim_forward(locosim_t* h, const float* d_action, float* d_dof, float* d_
     case 5: return locosim_configs31_forward(h, d_action, &o, s);
     default: return launch_forward<CfgPyrRK4>(h, d_action, o, s);
   }
+}
+int locosim_ray(locosim_t* h, const float* d_pnt, const float* d_vec, int n_rays, int frame, int frame_body,
+                int exclude_body, int flags, float* d_dist, int32_t* d_geom, float* d_normal, void* stream) {
+  if (!d_pnt || !d_vec || !d_dist || !d_geom) { h->err = "null buffer"; return 1; }
+  if (n_rays < 1) { h->err = "n_rays must be at least 1"; return 1; }
+  if (frame < LS_RAY_WORLD || frame > LS_RAY_TRACK) { h->err = "unknown ray frame"; return 1; }
+  if (flags & ~(LS_RAY_STATIC | LS_RAY_DYNAMIC | LS_RAY_PER_ENV)) { h->err = "unknown ray flag bits"; return 1; }
+  if (frame_body < 0 || frame_body >= h->hm.nb) { h->err = "frame_body out of range"; return 1; }
+  if (exclude_body < -1 || exclude_body >= h->hm.nb) { h->err = "exclude_body out of range"; return 1; }
+  if ((n_rays + LS_RAY_BLOCK - 1) / LS_RAY_BLOCK > 65535) { h->err = "too many rays per env for one launch grid"; return 1; }
+  const size_t n = (size_t)h->n_envs, nr = (size_t)n_rays, in = ((flags & LS_RAY_PER_ENV) ? n : 1) * nr * 12;
+  // the outputs are buffers 0-2; each is checked against the other outputs and against both inputs
+  const void* const buf_p[4] = {d_dist, d_geom, d_normal, d_pnt};
+  const void* const buf_v[4] = {d_dist, d_geom, d_normal, d_vec};
+  const size_t bytes[4] = {n * nr * 4, n * nr * 4, n * nr * 12, in};
+  if (buffers_overlap(buf_p, bytes, 4) || buffers_overlap(buf_v, bytes, 4)) {
+    h->err = "ray outputs overlap each other or the inputs"; return 1;
+  }
+  if (!locosim_ray_launch) { h->err = "the ray kernels are not compiled into this library"; return 1; }
+  if (n == 0) return 0;
+  CK(cudaSetDevice(h->device));
+  const RayArgs a = {d_pnt, d_vec, d_dist, d_geom, d_normal, n_rays, frame, frame_body, exclude_body, flags};
+  return locosim_ray_launch(h, &a, (cudaStream_t)stream);
 }
 int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {
   CK(cudaSetDevice(h->device));
@@ -2018,6 +2110,7 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
   if (damp) h->dm.has_damping = 1;
   CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
   if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (locosim_ray_sync_model && locosim_ray_sync_model(h)) return 1;
   CK(cudaMemset(h->st.dr_row, 0, (size_t)h->n_envs * 4));
   if (h->refout.key) {
     // (the reference keys name the envs' pool rows: every env is on row 0 of the new pool now)

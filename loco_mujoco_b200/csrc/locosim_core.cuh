@@ -3644,3 +3644,373 @@ LS_FN void reset_env(const int ms, const DevTask& t, EnvS<C>& e, int traj_no, in
   zero_applied(ms, e.env);
   SYNC();
 }
+
+// ----------------------------------------------------------------------------------------------------------
+// ray casting (locosim_ray): MuJoCo 2.3.7's mj_ray / engine_ray.c for the primitives, a GJK ray cast on the convex hull of
+// a mesh geom's vertices. One thread per ray; every routine works in the geom's frame (lp, lv: the ray's point and
+// direction there) and returns the distance in units of |lv| (-1: no hit) and an outward normal `ln` (not unit length).
+// ----------------------------------------------------------------------------------------------------------
+// one geom as the rays of one env see it: its world frame after kinematics() and what the routines read of the model
+struct RayGeom {
+  float pos[3], mat[9], size[3], rbound;
+  int type, body, vnum, sel;       // sel: LS_RAY_STATIC (no dof on the path to the world: MuJoCo's body_weldid 0) or LS_RAY_DYNAMIC
+  const float* verts;              // mesh: the hull vertices in the geom frame (mesh_vert)
+};
+
+template <class C>
+LS_DEV void ray_stage_geom(const int ms, const EnvS<C>& e, const int g, RayGeom& r) {
+  const DevModel& m = c_models[ms];
+  for (int k = 0; k < 3; k++) { r.pos[k] = e.gxpos[g][k]; r.size[k] = m.geom_size[3 * g + k]; }
+  geom_mat(ms, e, g, r.mat);
+  r.rbound = m.geom_rbound[g];
+  r.type = m.geom_type[g];
+  r.body = m.geom_bodyid[g];
+  r.sel = m.body_dofmask[r.body] == 0 ? LS_RAY_STATIC : LS_RAY_DYNAMIC;
+  r.vnum = r.type == LS_GEOM_MESH ? m.geom_meshnum[g] : 0;
+  r.verts = r.type == LS_GEOM_MESH ? m.mesh_vert + 3 * m.geom_meshadr[g] : nullptr;
+}
+
+// the ray of a query frame (LS_RAY_WORLD / BODY / HEADING / TRACK of body fb) in world coordinates
+template <class C>
+LS_DEV void ray_to_world(const EnvS<C>& e, const int frame, const int fb, const float* pnt, const float* vec, float* p,
+                         float* v) {
+  if (frame == LS_RAY_WORLD) {
+    for (int k = 0; k < 3; k++) { p[k] = pnt[k]; v[k] = vec[k]; }
+  } else if (frame == LS_RAY_BODY) {
+    rotvec(p, e.xquat[fb], pnt);
+    rotvec(v, e.xquat[fb], vec);
+    for (int k = 0; k < 3; k++) p[k] += e.xpos[fb][k];
+  } else if (frame == LS_RAY_HEADING) {
+    // yaw of the body's x axis; a vertical x axis has no heading: the world's then
+    const float* q = e.xquat[fb];
+    const float fx = 1 - 2 * (q[2] * q[2] + q[3] * q[3]), fy = 2 * (q[1] * q[2] + q[0] * q[3]);
+    const float h = sqrtf(fx * fx + fy * fy);
+    const float c = h > 1e-6f ? fx / h : 1.0f, s = h > 1e-6f ? fy / h : 0.0f;
+    p[0] = c * pnt[0] - s * pnt[1] + e.xpos[fb][0]; p[1] = s * pnt[0] + c * pnt[1] + e.xpos[fb][1]; p[2] = pnt[2] + e.xpos[fb][2];
+    v[0] = c * vec[0] - s * vec[1]; v[1] = s * vec[0] + c * vec[1]; v[2] = vec[2];
+  } else {
+    for (int k = 0; k < 3; k++) { p[k] = pnt[k] + e.xpos[fb][k]; v[k] = vec[k]; }
+  }
+}
+
+// roots x[0] <= x[1] of |p + x v|^2 = r2 over the first n coordinates, taken about the ray's point closest to the centre
+// (fp32 keeps its accuracy far from the geom there); returns the smaller non-negative root or -1 (MuJoCo's ray_quad)
+LS_DEV float ray_quad(const float* p, const float* v, const int n, const float r2, float* x) {
+  float a = 0, b = 0, q2 = 0;
+  for (int k = 0; k < n; k++) { a += v[k] * v[k]; b += p[k] * v[k]; }
+  x[0] = x[1] = -1;
+  if (a < LS_MINVAL) return -1;
+  const float t0 = -b / a;
+  for (int k = 0; k < n; k++) { const float q = p[k] + t0 * v[k]; q2 += q * q; }
+  if (q2 > r2) return -1;
+  const float d = sqrtf((r2 - q2) / a);
+  x[0] = t0 - d; x[1] = t0 + d;
+  return x[0] >= 0 ? x[0] : (x[1] >= 0 ? x[1] : -1);
+}
+
+// one-sided plane: hit from its +z side only, within size[0:2] where those are non-zero
+LS_DEV float ray_plane(const float* s, const float* lp, const float* lv, float* ln) {
+  if (lv[2] > -LS_MINVAL) return -1;
+  const float x = -lp[2] / lv[2];
+  if (x < 0) return -1;
+  const float p0 = lp[0] + x * lv[0], p1 = lp[1] + x * lv[1];
+  if ((s[0] > 0 && fabsf(p0) > s[0]) || (s[1] > 0 && fabsf(p1) > s[1])) return -1;
+  ln[0] = 0; ln[1] = 0; ln[2] = 1;
+  return x;
+}
+
+LS_DEV float ray_sphere(const float* s, const float* lp, const float* lv, float* ln) {
+  float xx[2];
+  const float x = ray_quad(lp, lv, 3, s[0] * s[0], xx);
+  for (int k = 0; k < 3; k++) ln[k] = lp[k] + x * lv[k];
+  return x;
+}
+
+LS_DEV float ray_ellipsoid(const float* s, const float* lp, const float* lv, float* ln) {
+  const float sp[3] = {lp[0] / s[0], lp[1] / s[1], lp[2] / s[2]}, sv[3] = {lv[0] / s[0], lv[1] / s[1], lv[2] / s[2]};
+  float xx[2];
+  const float x = ray_quad(sp, sv, 3, 1.0f, xx);
+  for (int k = 0; k < 3; k++) ln[k] = (lp[k] + x * lv[k]) / (s[k] * s[k]);
+  return x;
+}
+
+// the round side of a capsule or cylinder (radius s[0], half length s[1]): the first root within the flat ends
+LS_DEV void ray_round_side(const float* s, const float* lp, const float* lv, float& x, float* ln) {
+  float xx[2];
+  const float sol = ray_quad(lp, lv, 2, s[0] * s[0], xx);
+  if (sol >= 0 && fabsf(lp[2] + sol * lv[2]) <= s[1] && (x < 0 || sol < x)) {
+    x = sol;
+    ln[0] = lp[0] + sol * lv[0]; ln[1] = lp[1] + sol * lv[1]; ln[2] = 0;
+  }
+}
+
+LS_DEV float ray_capsule(const float* s, const float* lp, const float* lv, float* ln) {
+  float x = -1;
+  ray_round_side(s, lp, lv, x, ln);
+  for (int side = -1; side <= 1; side += 2) {           // hemispheres beyond the ends
+    const float dp[3] = {lp[0], lp[1], lp[2] - side * s[1]};
+    float xx[2];
+    ray_quad(dp, lv, 3, s[0] * s[0], xx);
+    for (int j = 0; j < 2; j++) {
+      if (xx[j] >= 0 && side * (lp[2] + xx[j] * lv[2]) >= s[1] && (x < 0 || xx[j] < x)) {
+        x = xx[j];
+        for (int k = 0; k < 3; k++) ln[k] = dp[k] + x * lv[k];
+      }
+    }
+  }
+  return x;
+}
+
+LS_DEV float ray_cylinder(const float* s, const float* lp, const float* lv, float* ln) {
+  float x = -1;
+  if (fabsf(lv[2]) > LS_MINVAL) {
+    for (int side = -1; side <= 1; side += 2) {
+      const float sol = (side * s[1] - lp[2]) / lv[2];
+      const float p0 = lp[0] + sol * lv[0], p1 = lp[1] + sol * lv[1];
+      if (sol >= 0 && p0 * p0 + p1 * p1 <= s[0] * s[0] && (x < 0 || sol < x)) {
+        x = sol; ln[0] = 0; ln[1] = 0; ln[2] = (float)side;
+      }
+    }
+  }
+  ray_round_side(s, lp, lv, x, ln);
+  return x;
+}
+
+LS_DEV float ray_box(const float* s, const float* lp, const float* lv, float* ln) {
+  float x = -1;
+  for (int i = 0; i < 3; i++) {
+    if (fabsf(lv[i]) <= LS_MINVAL) continue;
+    const int j = i == 0 ? 1 : 0, k = i == 2 ? 1 : 2;
+    for (int side = -1; side <= 1; side += 2) {
+      const float sol = (side * s[i] - lp[i]) / lv[i];
+      if (sol >= 0 && fabsf(lp[j] + sol * lv[j]) <= s[j] && fabsf(lp[k] + sol * lv[k]) <= s[k] && (x < 0 || sol < x)) {
+        x = sol; ln[0] = ln[1] = ln[2] = 0; ln[i] = (float)side;
+      }
+    }
+  }
+  return x;
+}
+
+// the hull cast runs in fp64: GJK's simplex steps lose fp32 accuracy near the hull's edges
+LS_DEV double dot3d(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+LS_DEV void cross3d(double* r, const double* a, const double* b) {
+  r[0] = a[1] * b[2] - a[2] * b[1]; r[1] = a[2] * b[0] - a[0] * b[2]; r[2] = a[0] * b[1] - a[1] * b[0];
+}
+// closest point to the origin of the triangle (a, b, c) (Ericson, Real-Time Collision Detection 5.1.5); `keep` gets the
+// vertices it is a combination of (bits 0-2)
+LS_DEV void hull_closest_tri(const double* a, const double* b, const double* c, double* cp, int& keep) {
+  double ab[3], ac[3];
+  for (int k = 0; k < 3; k++) { ab[k] = b[k] - a[k]; ac[k] = c[k] - a[k]; }
+  const double d1 = -dot3d(ab, a), d2 = -dot3d(ac, a);
+  if (d1 <= 0 && d2 <= 0) { for (int k = 0; k < 3; k++) cp[k] = a[k]; keep = 1; return; }
+  const double d3 = -dot3d(ab, b), d4 = -dot3d(ac, b);
+  if (d3 >= 0 && d4 <= d3) { for (int k = 0; k < 3; k++) cp[k] = b[k]; keep = 2; return; }
+  const double vc = d1 * d4 - d3 * d2;
+  if (vc <= 0 && d1 >= 0 && d3 <= 0) {
+    const double t = d1 / (d1 - d3);
+    for (int k = 0; k < 3; k++) cp[k] = a[k] + t * ab[k];
+    keep = 3; return;
+  }
+  const double d5 = -dot3d(ab, c), d6 = -dot3d(ac, c);
+  if (d6 >= 0 && d5 <= d6) { for (int k = 0; k < 3; k++) cp[k] = c[k]; keep = 4; return; }
+  const double vb = d5 * d2 - d1 * d6;
+  if (vb <= 0 && d2 >= 0 && d6 <= 0) {
+    const double t = d2 / (d2 - d6);
+    for (int k = 0; k < 3; k++) cp[k] = a[k] + t * ac[k];
+    keep = 5; return;
+  }
+  const double va = d3 * d6 - d5 * d4;
+  if (va <= 0 && d4 - d3 >= 0 && d5 - d6 >= 0) {
+    const double t = (d4 - d3) / ((d4 - d3) + (d5 - d6));
+    for (int k = 0; k < 3; k++) cp[k] = b[k] + t * (c[k] - b[k]);
+    keep = 6; return;
+  }
+  const double den = 1.0 / (va + vb + vc), v = vb * den, w = vc * den;
+  for (int k = 0; k < 3; k++) cp[k] = a[k] + v * ab[k] + w * ac[k];
+  keep = 7;
+}
+
+// v = the origin minus its closest point in conv(y[0..n)), n <= 4; y is reduced to the points that closest point needs
+LS_DEV void hull_closest(double (*y)[3], int& n, double* v) {
+  double cp[3];
+  int keep = 1;
+  if (n == 1) {
+    for (int k = 0; k < 3; k++) cp[k] = y[0][k];
+  } else if (n == 2) {
+    double d[3];
+    for (int k = 0; k < 3; k++) d[k] = y[1][k] - y[0][k];
+    const double dd = dot3d(d, d), t = dd > 0 ? -dot3d(y[0], d) / dd : 0.0f;
+    if (t <= 0) { keep = 1; for (int k = 0; k < 3; k++) cp[k] = y[0][k]; }
+    else if (t >= 1) { keep = 2; for (int k = 0; k < 3; k++) cp[k] = y[1][k]; }
+    else { keep = 3; for (int k = 0; k < 3; k++) cp[k] = y[0][k] + t * d[k]; }
+  } else if (n == 3) {
+    hull_closest_tri(y[0], y[1], y[2], cp, keep);
+  } else {
+    // tetrahedron: the closest of the faces whose plane separates the origin from the opposite vertex; none: inside
+    const int face[4][4] = {{0, 1, 2, 3}, {0, 2, 3, 1}, {0, 3, 1, 2}, {1, 3, 2, 0}};
+    double best = 3.0e38;
+    keep = 15;
+    cp[0] = cp[1] = cp[2] = 0;
+    for (int f = 0; f < 4; f++) {
+      const double *a = y[face[f][0]], *b = y[face[f][1]], *c = y[face[f][2]], *d = y[face[f][3]];
+      double ab[3], ac[3], nn[3];
+      for (int k = 0; k < 3; k++) { ab[k] = b[k] - a[k]; ac[k] = c[k] - a[k]; }
+      cross3d(nn, ab, ac);
+      double ad[3];
+      for (int k = 0; k < 3; k++) ad[k] = d[k] - a[k];
+      const double so = -dot3d(nn, a), sd = dot3d(nn, ad);
+      if (so * sd > 0) continue;                        // the origin is on the inner side of this face
+      double q[3];
+      int kf;
+      hull_closest_tri(a, b, c, q, kf);
+      const double dq = dot3d(q, q);
+      if (dq < best) {
+        best = dq;
+        for (int k = 0; k < 3; k++) cp[k] = q[k];
+        keep = 0;
+        for (int j = 0; j < 3; j++) if (kf & (1 << j)) keep |= 1 << face[f][j];
+      }
+    }
+  }
+  int m = 0;
+  for (int i = 0; i < n; i++)
+    if (keep & (1 << i)) { if (m != i) for (int k = 0; k < 3; k++) y[m][k] = y[i][k]; m++; }
+  n = m;
+  for (int k = 0; k < 3; k++) v[k] = -cp[k];
+}
+
+// index of the hull vertex farthest along d (the first of equals, like mpr_support_geom's scan)
+LS_DEV int hull_support(const float* vt, const int nv, const double* d) {
+  double mx = -3.0e38;
+  int best = 0;
+  for (int i = 0; i < nv; i++) {
+    const double t = d[0] * vt[3 * i] + d[1] * vt[3 * i + 1] + d[2] * vt[3 * i + 2];
+    if (t > mx) { mx = t; best = i; }
+  }
+  return best;
+}
+
+// GJK ray cast (van den Bergen, "Ray casting against general convex objects with application to continuous collision
+// detection", 2004) of s + x r against the hull of vt[0..nv) (bounding radius rb): the smallest x >= 0 on or in the hull, and
+// the outward normal of the support plane it stops at (zero when s itself is in the hull: x = 0). -1: a miss. tol: the
+// distance at which the point counts as on the hull.
+LS_DEV double hull_cast(const float* vt, const int nv, const double rb, const double* s, const double* r, const double tol,
+                        double* ln) {
+  double lam = 0, x[3] = {s[0], s[1], s[2]}, v[3], P[4][3], y[4][3];
+  int np = 0;
+  for (int k = 0; k < 3; k++) { v[k] = x[k] - vt[k]; ln[k] = 0; }
+  for (int it = 0; it < 64; it++) {
+    if (dot3d(v, v) <= tol * tol) break;
+    const float* pf = vt + 3 * hull_support(vt, nv, v);
+    const double p[3] = {pf[0], pf[1], pf[2]};
+    const double w[3] = {x[0] - p[0], x[1] - p[1], x[2] - p[2]};
+    const double vw = dot3d(v, w);
+    bool dup = false;
+    for (int i = 0; i < np; i++) dup |= P[i][0] == p[0] && P[i][1] == p[1] && P[i][2] == p[2];
+    if (vw > 0) {
+      const double vr = dot3d(v, r);
+      if (vr >= 0) return -1;
+      lam -= vw / vr;
+      for (int k = 0; k < 3; k++) { x[k] = s[k] + lam * r[k]; ln[k] = v[k]; }
+    } else if (dup) {
+      break;                                            // no support point left that moves x or v: x is on the hull
+    }
+    if (!dup) { for (int k = 0; k < 3; k++) P[np][k] = p[k]; np++; }
+    for (int i = 0; i < np; i++) for (int k = 0; k < 3; k++) y[i][k] = P[i][k] - x[k];
+    hull_closest(y, np, v);
+    for (int i = 0; i < np; i++) for (int k = 0; k < 3; k++) P[i][k] = y[i][k] + x[k];
+  }
+  // GJK reaches a face only linearly in fp32: where x stopped on three support points that span a face of the hull (no
+  // vertex beyond their plane), take the ray's crossing of that plane, and its normal, when it lies within the distance
+  // GJK left
+  // GJK reaches a face only linearly: where x stopped on three support points that span a face of the hull (no vertex
+  // beyond their plane), take the ray's crossing of that plane, and its normal, when it lies within the distance GJK left.
+  // np = 4: x ended in a tetrahedron of support points; of its faces that qualify, the ray enters the hull through the one
+  // it crosses last (at an edge, the other face's plane is crossed earlier)
+  const double rl = sqrt(dot3d(r, r)), left = 4 * sqrt(dot3d(v, v)) + tol, lam0 = lam;
+  bool refined = false;
+  for (int f = 0; f < (np == 4 ? 4 : (np == 3 ? 1 : 0)) && dot3d(ln, ln) > 0; f++) {
+    const double *a = P[f == 3 ? 1 : 0], *b = P[f == 2 ? 3 : (f == 3 ? 2 : 1)], *c = P[f == 1 ? 3 : (f == 3 ? 3 : 2)];
+    double e1[3], e2[3], n[3], d[3];
+    for (int k = 0; k < 3; k++) { e1[k] = b[k] - a[k]; e2[k] = c[k] - a[k]; d[k] = a[k] - s[k]; }
+    cross3d(n, e1, e2);
+    const double nr = dot3d(n, r), nn = sqrt(dot3d(n, n));
+    if (!(fabs(nr) > 1e-4 * nn * rl)) continue;
+    if (nr > 0) for (int k = 0; k < 3; k++) n[k] = -n[k];
+    const float* far = vt + 3 * hull_support(vt, nv, n);
+    if (n[0] * (far[0] - a[0]) + n[1] * (far[1] - a[1]) + n[2] * (far[2] - a[2]) > 1e-5 * nn * rb) continue;
+    const double l2 = dot3d(n, d) / dot3d(n, r);
+    if (fabs(l2 - lam0) * rl <= left && (!refined || l2 > lam)) {
+      lam = l2;
+      refined = true;
+      for (int k = 0; k < 3; k++) ln[k] = n[k];
+    }
+  }
+  return lam;
+}
+
+// a mesh geom: its hull. A ray that starts in the hull leaves it where the reversed ray, cast from beyond the bounding
+// sphere, enters it.
+LS_DEV float ray_mesh(const RayGeom& g, const float* lpf, const float* lvf, float* lnf) {
+  const double lp[3] = {lpf[0], lpf[1], lpf[2]}, lv[3] = {lvf[0], lvf[1], lvf[2]};
+  const double pl = sqrt(dot3d(lp, lp)), vl = sqrt(dot3d(lv, lv));
+  double ln[3];
+  double x = hull_cast(g.verts, g.vnum, g.rbound, lp, lv, 1e-9 * (pl + g.rbound), ln);
+  if (x == 0) {
+    const double T = (pl + 2 * g.rbound + 1e-3) / vl;
+    const double s2[3] = {lp[0] + T * lv[0], lp[1] + T * lv[1], lp[2] + T * lv[2]}, r2[3] = {-lv[0], -lv[1], -lv[2]};
+    const double back = hull_cast(g.verts, g.vnum, g.rbound, s2, r2, 1e-9 * (T * vl + g.rbound), ln);
+    x = back < 0 ? 0.0 : fmax(T - back, 0.0);
+  }
+  for (int k = 0; k < 3; k++) lnf[k] = (float)ln[k];
+  return (float)x;
+}
+
+// the world ray p + x v against the geoms G[0..ng) that `sel` (LS_RAY_STATIC | LS_RAY_DYNAMIC) selects, except those of body
+// `exclude`: the smallest x >= 0 (MuJoCo's mj_ray), its geom (-1 and x = -1: nothing is hit) and the unit outward normal
+// there, world frame (zeros for a miss). Bounding spheres (geom_rbound) reject most geoms first, as ray_eliminate does.
+LS_DEV float ray_geoms(const RayGeom* G, const int ng, const float* p, const float* v, const int exclude, const int sel,
+                       int* geom, float* nrm) {
+  float best = -1, bn[3] = {0, 0, 0};
+  int bg = -1;
+  const float vv = dot3(v, v);
+  if (vv > 0) {
+    for (int g = 0; g < ng; g++) {
+      const RayGeom& r = G[g];
+      if (!(r.sel & sel) || r.body == exclude) continue;
+      const float d[3] = {p[0] - r.pos[0], p[1] - r.pos[1], p[2] - r.pos[2]};
+      if (r.type != LS_GEOM_PLANE) {
+        const float rb = r.rbound * 1.0001f + 1e-6f, b = dot3(d, v), dd = dot3(d, d);
+        if (dd > rb * rb) {
+          if (b >= 0) continue;                         // outside, moving away
+          const float t0 = -b / vv, q[3] = {d[0] + t0 * v[0], d[1] + t0 * v[1], d[2] + t0 * v[2]};
+          if (dot3(q, q) > rb * rb) continue;
+          if (best >= 0 && t0 - rb / sqrtf(vv) > best) continue;   // the sphere lies beyond the nearest hit
+        }
+      }
+      float lp[3], lv[3], ln[3] = {0, 0, 0};
+      mulmatTvec3(lp, r.mat, d);
+      mulmatTvec3(lv, r.mat, v);
+      float x;
+      switch (r.type) {
+        case LS_GEOM_PLANE: x = ray_plane(r.size, lp, lv, ln); break;
+        case LS_GEOM_SPHERE: x = ray_sphere(r.size, lp, lv, ln); break;
+        case LS_GEOM_CAPSULE: x = ray_capsule(r.size, lp, lv, ln); break;
+        case LS_GEOM_ELLIPSOID: x = ray_ellipsoid(r.size, lp, lv, ln); break;
+        case LS_GEOM_CYLINDER: x = ray_cylinder(r.size, lp, lv, ln); break;
+        case LS_GEOM_BOX: x = ray_box(r.size, lp, lv, ln); break;
+        case LS_GEOM_MESH: x = ray_mesh(r, lp, lv, ln); break;
+        default: x = -1;
+      }
+      if (x >= 0 && (best < 0 || x < best)) {
+        best = x; bg = g;
+        mulmatvec3(bn, r.mat, ln);
+      }
+    }
+  }
+  const float nl = dot3(bn, bn);
+  const float inv = nl > 0 ? rsqrtf(nl) : 0.0f;
+  for (int k = 0; k < 3; k++) nrm[k] = bn[k] * inv;
+  *geom = bg;
+  return best;
+}

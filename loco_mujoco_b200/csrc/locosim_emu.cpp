@@ -37,6 +37,8 @@ struct EmuBase {
   virtual void dyn(const DynOut& o) = 0;
   virtual void fwd_out(const double* ctrl, const FwdOut& o) = 0;
   virtual int max_contacts() = 0;
+  virtual void ray(const float* pnt, const float* vec, int n_rays, int frame, int fb, int exclude, int flags, float* dist,
+                   int* geom, float* normal) = 0;
 };
 template <class C>
 struct EmuT : EmuBase {
@@ -122,6 +124,25 @@ struct EmuT : EmuBase {
     forward_dynamics(0, e, so, o);
   }
   int max_contacts() override { return C::MAXCON; }
+  void ray(const float* pnt, const float* vec, int n_rays, int frame, int fb, int exclude, int flags, float* dist, int* geom,
+           float* normal) override {
+    c_models[0] = m;
+    const bool bad = nonfinite_state(e, m.nv);
+    std::vector<RayGeom> G(m.ng);
+    if (!bad) {
+      kinematics(0, e);
+      for (int g = 0; g < m.ng; g++) ray_stage_geom(0, e, g, G[g]);
+    }
+    for (int k = 0; k < n_rays; k++) {
+      float p[3], v[3], nrm[3] = {0, 0, 0};
+      dist[k] = -1; geom[k] = -1;
+      if (!bad) {
+        ray_to_world(e, frame, fb, pnt + 3 * k, vec + 3 * k, p, v);
+        dist[k] = ray_geoms(G.data(), m.ng, p, v, exclude, flags, geom + k, nrm);
+      }
+      if (normal) for (int c = 0; c < 3; c++) normal[3 * k + c] = nrm[c];
+    }
+  }
   void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
 };
 
@@ -210,6 +231,14 @@ void emu_set_dof(EmuBase* s, float* out) {
 // as one control step of nsub sub-steps and leaves the list of its last sub-step there
 void emu_set_contact_list(EmuBase* s, int* ncon, float* con, int* id) {
   s->cl.ncon = ncon; s->cr.con = con; s->cr.id = id;
+}
+// ray casting (locosim_ray) of the emulated env's current state, with the model's own parameters: the rays pnt / vec fp32
+// [n_rays, 3] in `frame` of body fb, one at a time through the kernels' routines; dist fp32 [n_rays], geom int32 [n_rays],
+// normal fp32 [n_rays, 3] (may be NULL). No argument is checked here (locosim_ray checks them). Overwrites the env's
+// kinematics (not its state or warm start).
+void emu_ray(EmuBase* s, const float* pnt, const float* vec, int n_rays, int frame, int fb, int exclude, int flags,
+             float* dist, int* geom, float* normal) {
+  s->ray(pnt, vec, n_rays, frame, fb, exclude, flags, dist, geom, normal);
 }
 // the configuration's per-env contact cap (locosim_max_contacts)
 int emu_max_contacts(EmuBase* s) { return s->max_contacts(); }

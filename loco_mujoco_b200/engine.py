@@ -111,6 +111,8 @@ def load_library():
     lib.locosim_save_state.argtypes = [vp, vp, vp, vp]
     lib.locosim_load_state.restype = ip
     lib.locosim_load_state.argtypes = [vp, vp, ip, vp, vp, vp]
+    lib.locosim_ray.restype = ip
+    lib.locosim_ray.argtypes = [vp, vp, vp, ip, ip, ip, ip, ip, vp, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -127,7 +129,7 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_set_reference_outputs", "locosim_create_dataset_bodies", "locosim_inverse",
                     "locosim_create_dataset_inverse", "locosim_dynamics_terms", "locosim_forward", "locosim_state_words",
                     "locosim_save_state", "locosim_load_state", "locosim_max_contacts",
-                    "locosim_set_contact_list_outputs"]
+                    "locosim_set_contact_list_outputs", "locosim_ray"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -147,6 +149,11 @@ CONLIST_DIM = 19
 CONLIST_COLUMNS = dict(dist=(0, 1), pos=(1, 3), frame=(4, 9), force=(13, 6))
 CONLIST_ID_DIM = 5
 CONLIST_ID_COLUMNS = dict(geom=(0, 2), body=(2, 2), dim=(4, 1))
+# ray query frames and flags (include/locosim.h LS_RAY_*): where pnt / vec are given, and which geoms a ray can hit
+RAY_WORLD, RAY_BODY, RAY_HEADING, RAY_TRACK = 0, 1, 2, 3
+RAY_STATIC, RAY_DYNAMIC, RAY_PER_ENV = 1, 2, 4
+# rays per env of one locosim_ray launch: 65535 blocks of 128 (include/locosim.h)
+RAY_MAX = 65535 * 128
 
 
 
@@ -549,6 +556,45 @@ class CudaEngine:
                                              self._stream()))
         self.launches += 1
         return given
+
+    def ray(self, pnt, vec, dist, geom, normal=None, frame=RAY_WORLD, frame_body=0, exclude_body=-1,
+            flags=RAY_STATIC | RAY_DYNAMIC):
+        """Ray casting of include/locosim.h (locosim_ray, MuJoCo's mj_ray) against every env's geoms at its stored state:
+        the rays pnt + x vec, float32 cuda [n_rays, 3] for every env or, with RAY_PER_ENV in `flags`, [n_envs, n_rays, 3],
+        given in `frame` (RAY_WORLD, RAY_BODY, RAY_HEADING or RAY_TRACK) of body `frame_body`. Writes dist float32
+        [n_envs, n_rays] (the first hit in units of |vec|, -1: none), geom int32 [n_envs, n_rays] (the geom index, -1:
+        none) and, when given, normal float32 [n_envs, n_rays, 3] (unit outward normal at the hit, world frame). `flags`
+        selects RAY_STATIC (welded to the world: the floor) and / or RAY_DYNAMIC (the robot's) geoms; the geoms of body
+        `exclude_body` (-1: none) are skipped. The outputs must not overlap each other or the inputs. Changes nothing in
+        the engine; stream-ordered, no allocation (can be captured in a CUDA graph)."""
+        n = self.n_envs
+        if frame not in (RAY_WORLD, RAY_BODY, RAY_HEADING, RAY_TRACK):
+            raise ValueError("unknown ray frame %r" % (frame,))
+        if int(flags) & ~(RAY_STATIC | RAY_DYNAMIC | RAY_PER_ENV):
+            raise ValueError("unknown ray flag bits in %r" % (flags,))
+        if not 0 <= int(frame_body) < self.nbody:
+            raise ValueError("frame_body %r out of range [0, %d)" % (frame_body, self.nbody))
+        if not -1 <= int(exclude_body) < self.nbody:
+            raise ValueError("exclude_body %r out of range [-1, %d)" % (exclude_body, self.nbody))
+        shape = getattr(pnt, "shape", None)
+        if shape is None or len(shape) < 2:
+            raise ValueError("pnt must be a float32 tensor [n_rays, 3] or [n_envs, n_rays, 3]")
+        r = int(shape[-2])
+        if not 1 <= r <= RAY_MAX:
+            raise ValueError("n_rays %d out of range [1, %d]" % (r, RAY_MAX))
+        ins = (n, r, 3) if int(flags) & RAY_PER_ENV else (r, 3)
+        spans = (("pnt", pnt, ins), ("vec", vec, ins), ("dist", dist, (n, r)), ("geom", geom, (n, r)),
+                 ("normal", normal, (n, r, 3)))
+        for name, x, shp in spans:
+            if x is not None or name != "normal":
+                self._check_tensor(x, name, shp, "int32" if name == "geom" else "float32")
+        # the inputs may share memory with each other; every output is checked against everything else
+        self._check_disjoint(spans[2:] + spans[:1])
+        self._check_disjoint(spans[2:] + spans[1:2])
+        self._check(self.lib.locosim_ray(self.h, _ptr(pnt), _ptr(vec), r, int(frame), int(frame_body), int(exclude_body),
+                                         int(flags), _ptr(dist), _ptr(geom), _ptr(normal), self._stream()))
+        self.launches += 1
+        return dist, geom, normal
 
     @property
     def state_layout(self):

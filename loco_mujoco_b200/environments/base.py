@@ -178,6 +178,9 @@ class LocoEnv:
         self._collision_groups = list(collision_groups) if collision_groups else []
         self._domain_rand_config = domain_randomization_config
         self._domain_rand_pool_size = viewer_params.pop("domain_randomization_pool_size", 64)
+        # render(): the reference's viewer settings that a headless frame uses (camera_params["follow"], width, height)
+        self._camera_params = dict(viewer_params.get("camera_params") or {})
+        self._render_size = (int(viewer_params.get("width", 640)), int(viewer_params.get("height", 480)))
         self._domain_rand = None
         self._timestep = timestep
         self._n_substeps = n_substeps
@@ -807,6 +810,150 @@ class LocoEnv:
         return out, {k: out[k] if want[k] else None for k in names}
 
     # ---------------------------------------------------------------------------------------------------
+    # ray casting (MuJoCo's mj_ray, include/locosim.h locosim_ray) and cameras built on it
+    # ---------------------------------------------------------------------------------------------------
+    RAY_MODES = dict(world=0, body=1, heading=2, track=3)
+
+    def _body_arg(self, body, what):
+        if isinstance(body, str):
+            return self.body_index(body)
+        b = int(body)
+        if not 0 <= b < self._model.nbody:
+            raise ValueError("%s %r out of range [0, %d)" % (what, body, self._model.nbody))
+        return b
+
+    def ray_cast(self, pnt, vec, frame=None, mode="world", exclude_body=None, static=True, dynamic=True, normal=False,
+                 out=None):
+        """MuJoCo's mj_ray for every env at its current state, the state of info["next_obs"]: the rays pnt + x vec (float32
+        torch tensors on the env's device, [n_rays, 3] for the same rays in every env or [num_envs, n_rays, 3] per env)
+        against the env's geoms. `mode` says where the rays are given, relative to body `frame` (a name or an index; the
+        root body, index 1, when None):
+            "world"    world coordinates (`frame` is not used)
+            "body"     the body's frame (position and orientation of body_state)
+            "heading"  at the body's origin, turned by the yaw of its x axis only (level height scans that turn with it)
+            "track"    at the body's origin with the world's axes
+        `static` selects the geoms welded to the world (the floor), `dynamic` the robot's; the geoms of body `exclude_body`
+        (name or index) are skipped. Returns a dict of tensors on the env's device:
+            dist    float32 [num_envs, n_rays]     the first hit in units of |vec| (metres for a unit vec), -1 for none
+            geom    int32 [num_envs, n_rays]       its geom (`geom_index`, `geom_names`), -1 for none
+            normal  float32 [num_envs, n_rays, 3]  (normal=True) the unit outward surface normal there, world frame
+        Primitives follow MuJoCo 2.3.7 (one-sided planes; a ray that starts inside a geom reports where it leaves it); a
+        mesh is hit on the convex hull of its vertices, the shape the engine collides with. A non-finite state gives that
+        env -1. `out`: the dict of an earlier call, filled in place (a graph-captured loop then allocates nothing). Changes
+        nothing in the env."""
+        import torch
+        from ..engine import RAY_STATIC, RAY_DYNAMIC, RAY_PER_ENV
+        eng = self._get_engine()
+        if mode not in self.RAY_MODES:
+            raise ValueError("mode must be one of %s" % ", ".join(self.RAY_MODES))
+        fb = 0 if mode == "world" else (1 if frame is None else self._body_arg(frame, "frame"))
+        ex = -1 if exclude_body is None else self._body_arg(exclude_body, "exclude_body")
+        if not isinstance(pnt, torch.Tensor) or pnt.dim() not in (2, 3):
+            raise ValueError("pnt must be a float32 torch tensor [n_rays, 3] or [num_envs, n_rays, 3]")
+        flags = (RAY_STATIC if static else 0) | (RAY_DYNAMIC if dynamic else 0) | (RAY_PER_ENV if pnt.dim() == 3 else 0)
+        n, r = self.num_envs, int(pnt.shape[-2])
+        if out is None:
+            out = {}
+        elif not isinstance(out, dict):
+            raise ValueError("out must be the dict of an earlier ray_cast() call")
+        shapes = dict(dist=((n, r), torch.float32), geom=((n, r), torch.int32), normal=((n, r, 3), torch.float32))
+        for k, (shape, dtype) in shapes.items():
+            if (k != "normal" or normal) and (out.get(k) is None or tuple(out[k].shape) != shape):
+                out[k] = torch.empty(shape, dtype=dtype, device=eng.device)
+        eng.ray(pnt, vec, out["dist"], out["geom"], out["normal"] if normal else None, frame=self.RAY_MODES[mode],
+                frame_body=fb, exclude_body=ex, flags=flags)
+        return out
+
+    def camera(self, width, height, fovy=45.0, mode="follow", body=None, distance=3.5, elevation=-20.0, azimuth=90.0,
+               pos=None, quat=None, normal=False, out=None):
+        """Depth and segmentation images of every env from one pinhole camera (one ray per pixel, row-major, pixel (0, 0)
+        at the top left; `fovy` in degrees is the angle between the top and bottom image edges):
+            "follow"  looks at the origin of `body` (the root when None) from `distance` metres, at `elevation` and
+                      `azimuth` degrees (MuJoCo's free camera: elevation < 0 looks down), with the world's axes: the
+                      camera_params["follow"] of the reference's viewer
+            "body"    fixed to `body` at `pos` (3) with orientation `quat` (w x y z) in its frame, looking along the
+                      camera frame's -z with y up (MuJoCo's camera convention): an egocentric camera
+        Returns a dict of tensors on the env's device:
+            depth   float32 [num_envs, height, width]     distance along the optical axis (metres), inf where nothing is hit
+            geom    int32 [num_envs, height, width]       the geom seen, -1 for none
+            body    int32 [num_envs, height, width]       its body (`body_index`), -1 for none
+            normal  float32 [num_envs, height, width, 3]  (normal=True) unit surface normal, world frame
+        and the ray set it cast: pnt / vec (the rays in the query frame, vec of unit length), dist (metres along each ray,
+        -1 for none). `out`: the dict of an earlier call with
+        the same arguments, filled in place."""
+        import math
+        import torch
+        eng = self._get_engine()
+        W, H = int(width), int(height)
+        if W < 1 or H < 1:
+            raise ValueError("width and height must be positive")
+        if mode not in ("follow", "body"):
+            raise ValueError('mode must be "follow" or "body"')
+        b = 1 if body is None else self._body_arg(body, "body")
+        dev = eng.device
+        if out is None or out.get("_key") != (W, H, fovy, mode, b, distance, elevation, azimuth, str(pos), str(quat)):
+            out = {} if out is None else out
+            t = math.tan(math.radians(float(fovy)) / 2)
+            jj, ii = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64),
+                                    indexing="ij")
+            u = (ii + 0.5 - W / 2) / (H / 2) * t
+            v = (H / 2 - jj - 0.5) / (H / 2) * t
+            if mode == "follow":
+                az, el = math.radians(float(azimuth)), math.radians(float(elevation))
+                fwd = torch.tensor([math.cos(el) * math.cos(az), math.cos(el) * math.sin(az), math.sin(el)],
+                                   dtype=torch.float64)
+                up = torch.tensor([-math.sin(el) * math.cos(az), -math.sin(el) * math.sin(az), math.cos(el)],
+                                  dtype=torch.float64)
+                origin = -float(distance) * fwd
+            else:
+                from ..mjcf import quat_to_mat
+                R = torch.tensor(np.asarray(quat_to_mat(np.asarray([1.0, 0, 0, 0] if quat is None else quat,
+                                                                   dtype=np.float64))), dtype=torch.float64)
+                fwd, up = -R[:, 2], R[:, 1]
+                origin = torch.tensor([0.0, 0, 0] if pos is None else [float(x) for x in pos], dtype=torch.float64)
+            right = torch.linalg.cross(fwd, up)
+            d = fwd + u[..., None] * right + v[..., None] * up
+            d = d / d.norm(dim=-1, keepdim=True)
+            out["vec"] = d.reshape(-1, 3).to(torch.float32).to(dev)
+            out["pnt"] = origin.expand(H * W, 3).to(torch.float32).contiguous().to(dev)
+            out["_cos"] = (d @ fwd).to(torch.float32).reshape(H, W).to(dev)
+            out["_key"] = (W, H, fovy, mode, b, distance, elevation, azimuth, str(pos), str(quat))
+            out.pop("_rays", None)
+        rays = self.ray_cast(out["pnt"], out["vec"], frame=b, mode="track" if mode == "follow" else "body", normal=normal,
+                             out=out.get("_rays"))
+        out["_rays"] = rays
+        n = self.num_envs
+        dist, geom = rays["dist"].view(n, H, W), rays["geom"].view(n, H, W)
+        if out.get("_bodyid") is None:
+            out["_bodyid"] = torch.tensor(np.asarray(self._model.geom_bodyid), dtype=torch.int32, device=dev)
+        out["dist"], out["geom"] = dist, geom
+        out["depth"] = torch.where(dist >= 0, dist * out["_cos"], torch.full_like(dist, float("inf")))
+        out["body"] = torch.where(geom >= 0, out["_bodyid"][geom.clamp(min=0).long()], geom)
+        if normal:
+            out["normal"] = rays["normal"].view(n, H, W, 3)
+        return out
+
+    def _body1_origin(self, env):
+        """World position of body 1 (the root) of env `env` at its stored state, from its own joints (kin_body of the
+        engine's kinematics in fp64 on the host): where render() puts the floor's checker squares."""
+        from ..mjcf import quat_to_mat
+        m = self._model
+        q = self._get_engine().get_state()[0][int(env)].double().cpu().numpy()
+        pos, quat = np.asarray(m.body_pos[1], dtype=np.float64).copy(), np.asarray(m.body_quat[1], dtype=np.float64)
+        R = np.asarray(quat_to_mat(quat))
+        for j in range(m.body_jntadr[1], m.body_jntadr[1] + m.body_jntnum[1]):
+            x = q[j] - m.qpos0[j]
+            axis, anchor = R @ np.asarray(m.jnt_axis[j]), pos + R @ np.asarray(m.jnt_pos[j])
+            if m.jnt_type[j] == mjcf.JNT_SLIDE:
+                pos = pos + axis * x
+            else:
+                c, s = np.cos(x), np.sin(x)
+                K = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
+                Rj = np.eye(3) + s * K + (1 - c) * K @ K
+                pos, R = anchor + Rj @ (pos - anchor), Rj @ R
+        return pos
+
+    # ---------------------------------------------------------------------------------------------------
     # saved states (MuJoCo's mj_copyData for a batch, include/locosim.h locosim_save_state / locosim_load_state)
     # ---------------------------------------------------------------------------------------------------
     def save_state(self, out=None):
@@ -996,8 +1143,45 @@ class LocoEnv:
     def stop(self):
         pass
 
-    def render(self, record=False):
-        raise NotImplementedError("rendering is out of scope (headless engine)")
+    def render(self, record=False, env=0):
+        """A frame of env `env` from the follow camera, shaded in torch from one `camera()` call: a flat colour per body with
+        Lambert shading on the surface normal, a checker floor, and a sky colour where nothing is hit. Returns uint8 numpy
+        [width, height, 3], the layout of the reference's render(True) (GymnasiumWrapper swaps it to [height, width, 3]).
+        The camera is camera_params["follow"] (distance, elevation, azimuth in degrees, looking at the root body), else
+        distance 3.5, elevation -20, azimuth 90; the size is the width / height keyword arguments of the env, else 640 x
+        480. The engine is headless: the frame is returned whether or not `record` is set, and nothing is displayed.
+        Textures, visual-only geoms and shadows are not drawn. The query casts the camera's rays for every env of the
+        batch, so its cost grows with num_envs."""
+        import torch
+        if not 0 <= int(env) < self.num_envs:
+            raise ValueError("env %r out of range [0, %d)" % (env, self.num_envs))
+        follow = dict(distance=3.5, elevation=-20.0, azimuth=90.0)
+        follow.update(self._camera_params.get("follow", {}))
+        W, H = self._render_size
+        cam = self.camera(W, H, mode="follow", distance=follow["distance"], elevation=follow["elevation"],
+                          azimuth=follow["azimuth"], normal=True)
+        i = int(env)
+        geom, body, nrm = cam["geom"][i], cam["body"][i], cam["normal"][i]
+        dirs = cam["vec"].view(H, W, 3)
+        hit = geom >= 0
+        # sky: lighter towards the horizon
+        up = dirs[..., 2].clamp(-1, 1)
+        sky = torch.stack([0.55 + 0.25 * (1 - up), 0.7 + 0.2 * (1 - up), 0.95 + 0.0 * up], dim=-1)
+        # flat body colours from a fixed palette; the floor (static geoms) as a 0.5 m checker
+        palette = torch.tensor([[0.85, 0.45, 0.25], [0.3, 0.55, 0.85], [0.9, 0.8, 0.3], [0.45, 0.75, 0.4],
+                                [0.75, 0.4, 0.7], [0.4, 0.75, 0.75], [0.85, 0.6, 0.6], [0.6, 0.6, 0.85]],
+                               device=geom.device)
+        base = palette[body.clamp(min=0) % len(palette)]
+        eye = torch.as_tensor(self._body1_origin(i), dtype=torch.float32, device=geom.device) + cam["pnt"][0]
+        point = eye + cam["dist"][i].clamp(min=0)[..., None] * dirs
+        checker = ((torch.floor(point[..., 0] / 0.5) + torch.floor(point[..., 1] / 0.5)) % 2)[..., None]
+        floor = 0.55 + 0.25 * checker.expand(-1, -1, 3)
+        base = torch.where((body == 0)[..., None], floor, base)
+        sun = torch.tensor([0.3, 0.2, 0.93], device=geom.device)
+        sun = sun / sun.norm()
+        lambert = (0.35 + 0.45 * (nrm @ sun).clamp(min=0) + 0.2 * (-(nrm * dirs).sum(-1)).clamp(min=0))[..., None]
+        rgb = torch.where(hit[..., None], base * lambert, sky).clamp(0, 1)
+        return (rgb * 255).round().to(torch.uint8).transpose(0, 1).contiguous().cpu().numpy()
 
     # ---------------------------------------------------------------------------------------------------
     # observation bookkeeping (reference: base.py:257-276, 729-775)
@@ -1150,7 +1334,8 @@ class LocoEnv:
         """Kinematic replay (no physics is advanced in the reference either: base.py:314-386)."""
         assert self.trajectories is not None
         if render or record:
-            raise NotImplementedError("rendering is out of scope (headless engine)")
+            raise NotImplementedError("play_trajectory(render=True / record=True) needs a viewer and a video writer, which "
+                                      "this headless engine does not have: call render() after each step instead")
         big = np.iinfo(np.int32).max
         n_episodes = big if n_episodes is None else n_episodes
         n_steps_per_episode = big if n_steps_per_episode is None else n_steps_per_episode

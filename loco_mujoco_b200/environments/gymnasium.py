@@ -55,7 +55,13 @@ class GymnasiumWrapper(_Base):
         return self._env.reset(), {}
 
     def render(self):
-        return self._env.render()
+        """render_mode "rgb_array": the env's frame as uint8 [height, width, 3] (the reference's swap of render(True)'s
+        [width, height, 3]). "human" needs a window, which this headless engine does not have."""
+        if self.render_mode == "rgb_array":
+            return np.swapaxes(self._env.render(True), 0, 1)
+        if self.render_mode == "human":
+            raise NotImplementedError("render_mode 'human' needs a viewer window: the engine is headless, use 'rgb_array'")
+        return None
 
     def close(self):
         self._env.stop()

@@ -317,6 +317,7 @@ class HumanoidTorque4AgesAll:
     forward_dynamics = _unavailable("the forward dynamics (forward_dynamics)")
     save_state = _unavailable("saved states (save_state)")
     load_state = _unavailable("saved states (load_state)")
+    ray_cast = camera = render = _unavailable("ray casting (ray_cast / camera / render)")
 
     def _scatter(self, parts):
         """Per-humanoid tensors [n_k, ...] -> one tensor in env order (env i = humanoid i % 4, its (i // 4)-th env)."""

@@ -60,7 +60,9 @@ class UnitreeA1(LocoEnv):
             xml_handle = None
         collision_groups = [("floor", ["floor"]), ("foot_FR", ["FR_foot"]), ("foot_FL", ["FL_foot"]),
                             ("foot_RR", ["RR_foot"]), ("foot_RL", ["RL_foot"])]      # unitreeA1.py:223-227
-        super().__init__(xml_handle, action_spec, observation_spec, collision_groups, **kwargs)
+        if camera_params is None:
+            camera_params = dict(follow=dict(distance=3.5, elevation=-20.0, azimuth=90.0))   # unitreeA1.py:239-241
+        super().__init__(xml_handle, action_spec, observation_spec, collision_groups, camera_params=camera_params, **kwargs)
 
     # -- observation layout -------------------------------------------------------------------------------
     def _get_observation_space(self):

@@ -21,7 +21,8 @@ def make_sharded(task_id, n_total, rank=None, world_size=None, device=None, seed
     Its `xfrc_applied` / `qfrc_applied`, `body_state` / `next_body_state`, `reference_body_state` /
     `next_reference_body_state`, `contact_wrench`, `dof_outputs` and `contacts`, what `inverse_dynamics(qacc)` and
     `forward_dynamics(action)` take and return and what `dynamics_terms()` returns hold the rows of this shard's envs only
-    (global env offset + i is row i). So does `save_state()`; its rows load into any shard of the same task."""
+    (global env offset + i is row i). So does `save_state()`; its rows load into any shard of the same task. So do
+    `ray_cast(...)` and `camera(...)`, and `render(env=i)` draws this shard's env i."""
     from . import LocoEnv
     rank = dist.get_rank() if rank is None else rank
     world_size = dist.get_world_size() if world_size is None else world_size
@@ -143,7 +144,8 @@ class MixedBatch:
     So are body outputs: `envs[i].body_state` / `envs[i].next_body_state`, reference outputs:
     `envs[i].reference_body_state` / `envs[i].next_reference_body_state`, contact outputs: `envs[i].contact_wrench`, dof
     outputs: `envs[i].dof_outputs`, the contact list: `envs[i].contacts`, inverse dynamics: `envs[i].inverse_dynamics(qacc)` / `envs[i].dof_index(joint)`,
-    dynamics terms: `envs[i].dynamics_terms(...)`, forward dynamics: `envs[i].forward_dynamics(action, ...)`, and saved
+    dynamics terms: `envs[i].dynamics_terms(...)`, forward dynamics: `envs[i].forward_dynamics(action, ...)`, ray casting:
+    `envs[i].ray_cast(...)` / `envs[i].camera(...)` / `envs[i].render(env=k)`, and saved
     states: `engines[i].save_state(engines[i].next_obs)` / `engines[i].load_state(rows, index, engines[i].next_obs)` (`step`
     drives the engines, so a member's observation to act on next is its engine's `next_obs`).
     """
