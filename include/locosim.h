@@ -132,6 +132,45 @@ int locosim_nbody(const locosim_t* h);
  * it is replayed. */
 int locosim_set_applied_forces(locosim_t* h, float* d_xfrc, float* d_qfrc);
 
+/* Terrain (height field) origin per env. A model packed with a terrain (include/locosim_modelpack.h: UnitreeA1 only; any other
+ * model with a terrain is refused at create) runs on the kernel configuration CfgEllEulerTerrain. Semantics, MuJoCo 2.3.7's
+ * hfield geom and mjc_ConvexHField as this project defines them:
+ *   Shape: nrow x ncol samples (nrow, ncol >= 2), size = (rx, ry, elevation, base). Sample (r, c) sits at
+ *     x = c * 2 rx / (ncol - 1) - rx, y = r * 2 ry / (nrow - 1) - ry, z = data[r * ncol + c] * elevation in the geom's frame
+ *     (data normalised to [0, 1], as MuJoCo's compiler stores it); the solid reaches down to z = -base. One field per model,
+ *     unrotated (a geom quaternion other than identity is refused).
+ *   Prisms: each cell (r, c) is split into two triangles, extruded down to -base: triangle 0 = grid points (c, r), (c, r+1),
+ *     (c+1, r), triangle 1 = (c, r+1), (c+1, r), (c+1, r+1), i.e. the diagonal from (c+1, r) to (c, r+1), the triangles of
+ *     MuJoCo's strip builder in mjc_ConvexHField as this project restates it (MuJoCo's source could not be checked here:
+ *     this is THIS PROJECT'S DEFINITION, used by collision, the fp64 reference and the ray caster alike). A prism's six
+ *     vertices are ordered bottom (z = -base) then top, each in the triangle's order; its support is the first maximum of
+ *     the six, its centre (MPR's first portal point) their mean.
+ *   Collision of the terrain with a robot geom g (sphere, capsule, cylinder or box): g is expressed in the field's frame; its
+ *     bounding box comes from its support along +-x, +-y, +-z; the pair ends when that box, grown by the pair's margin,
+ *     misses the field's box [-rx, rx] x [-ry, ry] x [-base, elevation]. The cell range is floor / ceil of the grown box's
+ *     grid coordinates, clamped to the grid. Prisms are taken in (row, column, triangle) order; one whose three top points
+ *     all lie below (lowest point of g) - margin is skipped; every other one runs MPR (the engine's mjc_Convex) with each
+ *     side inflated by margin / 2, and each one that penetrates gives one contact: dist = margin - depth, the MPR normal
+ *     (from the terrain into g) and position, as for every convex pair. At most 50 contacts per pair (mjMAXCONPAIR); the
+ *     margin handling is this project's definition too.
+ *   Contact parameters: the terrain geom carries the floor geom's contype / conaffinity, friction, condim, solref, solimp,
+ *     solmix, priority, margin and gap; it is paired with exactly the geoms the floor is paired with, and it is geom1 of
+ *     those pairs. The terrain pairs come after every other pair. The floor plane stays: a terrain above the floor hides it,
+ *     a pit can reach down to it.
+ *   Origin: env i sees the field translated by (-origin[i][0], -origin[i][1], 0): origin[i] is the terrain point (x, y) under
+ *     env i's world origin, its reset spot. Resets are unchanged (root x / y zeroed, root z from the dataset): it is the
+ *     terrain's job to be flat at height 0 under every spawn point (loco_mujoco_b200/terrain.py builds such fields). The
+ *     termination test is unchanged too: UnitreeA1's q_trunk_tz > -0.24 ends an episode in a pit deeper than 0.24 m.
+ * d_origin: caller-owned fp32 [n_envs, 2], read by every later step and on-demand query (locosim_inverse, locosim_forward,
+ * locosim_dynamics_terms, ...). NULL = all zeros = the state after locosim_create. Like the applied-force buffers, the origin is
+ * not part of a saved state row: index it with the same rows. Register outside of stream capture, like
+ * locosim_set_applied_forces. Refused on a handle without a terrain. locosim_create_dataset_inverse evaluates dataset rows, not
+ * envs: they take the zero origin.
+ *   Rays (locosim_ray): the terrain is a static geom of the world body (LS_RAY_STATIC; excluded with exclude_body 0), cast
+ *     in env i's translated frame as mj_rayHfield: the top triangles (the diagonal above), the four sides up to the
+ *     surface along the edge, and the base; the first hit of any of them, with its outward normal. */
+int locosim_set_terrain_origin(locosim_t* h, float* d_origin);
+
 /* Body outputs, MuJoCo's per-body kinematics (what a loco-mujoco user reads from env._data: xpos, xquat, body velocities):
  * caller-owned DEVICE buffers, each fp32 [n_envs, nbody, LS_BODY_DIM]. Per body (row) 13 values:
  *   xpos (3)  world position of the body frame

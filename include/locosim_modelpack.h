@@ -21,18 +21,21 @@
 enum {
   MPI_MAGIC = 0, MPI_VERSION, MPI_NBODY, MPI_NV, MPI_NGEOM, MPI_NU, MPI_NPAIR, MPI_NMESHVERT,
   MPI_INTEGRATOR /*0 Euler,1 RK4*/, MPI_CONE /*0 pyramidal,1 elliptic*/, MPI_ITERATIONS,
+  MPI_HF_NROW /*height field rows, 0 = no terrain*/, MPI_HF_NCOL /*height field columns*/,
   MPI_HEADER_LEN = 16
 };
 /* real header slots */
 enum {
   MPR_TIMESTEP = 0, MPR_GRAV_X, MPR_GRAV_Y, MPR_GRAV_Z, MPR_IMPRATIO, MPR_TOLERANCE, MPR_MEANINERTIA,
+  MPR_HF_SIZE /*4 slots: the height field's size (rx, ry, elevation, base)*/,
   MPR_HEADER_LEN = 16
 };
 
 /* X(name, count-expression) ; nb=nbody nv=nv ng=ngeom nu=nu np=npair nm=nmeshvert
  * pair_geom: candidate geom pairs (g1, g2) with type(g1) <= type(g2); the pairs handled by a dedicated primitive routine
  * (plane-X, sphere-sphere, sphere-capsule, capsule-capsule, sphere-box) MUST come first, the general convex pairs
- * (mjc_Convex / MPR) last; model order inside each part (loco_mujoco_b200/modelpack.py pack()). */
+ * (mjc_Convex / MPR) next, and the pairs (terrain, g) of the height field last (none without a terrain); model order
+ * inside each part (loco_mujoco_b200/modelpack.py pack()). */
 #define LOCOSIM_MP_INT_FIELDS(X) \
   X(body_parentid, nb) X(body_jntadr, nb) X(body_jntnum, nb) X(body_lastdof, nb) X(body_rootid, nb) \
   X(jnt_type, nv) X(jnt_bodyid, nv) X(jnt_limited, nv) X(dof_parentid, nv) \
@@ -53,6 +56,12 @@ enum {
   X(mesh_vert, 3 * nm) \
   X(actuator_gear, nu) X(actuator_ctrlrange, 2 * nu) X(actuator_forcerange, 2 * nu) X(actuator_gain, nu) \
   X(actuator_bias, 3 * nu)
+
+/* Height field (terrain): present when ints[MPI_HF_NROW] > 0. Its elevation samples follow the real fields as one
+ * trailing array, hfield_data[nrow * ncol] (row major, normalised to [0, 1]); its size is reals[MPR_HF_SIZE .. + 4). The
+ * terrain is the model's LAST geom (type LS_GEOM_HFIELD, on the world body). A pack without a terrain has zeros in these
+ * slots and no trailing array: it is the same bytes as before the terrain existed, and keeps LOCOSIM_MP_VERSION.
+ * The terrain's semantics are include/locosim.h's (locosim_set_terrain_origin). */
 
 /* geom / joint type codes (MuJoCo's numbering) */
 enum { LS_GEOM_PLANE = 0, LS_GEOM_HFIELD, LS_GEOM_SPHERE, LS_GEOM_CAPSULE, LS_GEOM_ELLIPSOID, LS_GEOM_CYLINDER,

@@ -1038,6 +1038,11 @@ __global__ void __launch_bounds__(32) dataset_body_kernel(int ms, DevTask t, con
 // ----------------------------------------------------------------------------------------------------------
 // pk: the handle's staged pair table in global memory (the source of the step kernels' TMA copy, whose layout DevModel::pk_n
 // then describes), or NULL: the model's table
+// EnvS::env of dataset row r in inverse_kernel: the row itself, which no per-env buffer is indexed with on that path; the
+// terrain unit (locosim_terrain.cu) marks it as no env (-1 - r), so that the terrain pass takes the zero origin there
+#ifndef LS_DATASET_ENV
+#define LS_DATASET_ENV(r) (r)
+#endif
 template <class C>
 LS_DEV void inverse_setup(const int ms, EnvS<C>& e, const float* prm, const int env, const int* pk) {
   if ((threadIdx.x & 31) == 0) {
@@ -1075,7 +1080,7 @@ __global__ void __launch_bounds__(32) inverse_kernel(int ms, EngineState st, Dev
   if (inv_dt > 0.0f) {
     const int per = t.traj_len - 1, tj = r / per, sp = r - tj * per, ncol = 2 * nv + t.n_goal;
     const float* row = t.table + ((size_t)tj * t.traj_len + sp) * ncol;
-    inverse_setup(ms, e, prm, r, pk);
+    inverse_setup(ms, e, prm, LS_DATASET_ENV(r), pk);
     for (int i = lane; i < nv; i += 32) {
       e.qpos[i] = reset_value(t, row, nv, LS_OBS_QPOS, i, 0.0f);
       e.qvel[i] = reset_qvel0(t, row, nv, i);
@@ -1200,6 +1205,9 @@ __global__ void __launch_bounds__(LS_RAY_BLOCK) ray_kernel(int ms, EngineState s
     float p[3], v[3];
     ray_to_world(e, a.frame, a.frame_body, pnt, vec, p, v);
     dist = ray_geoms(G, ng, p, v, a.exclude, a.flags, &geom, nrm);
+#ifdef LOCOSIM_TERRAIN
+    if constexpr (C::TERRAIN) ray_terrain(ms, r, p, v, a.exclude, a.flags, &dist, &geom, nrm);
+#endif
   }
   a.dist[o] = dist;
   a.geom[o] = geom;
@@ -1270,6 +1278,7 @@ struct locosim_handle {
   int* d_mints = nullptr; float* d_mreals = nullptr; int* d_tints = nullptr; float* d_treals = nullptr;
   float* d_pool = nullptr;
   unsigned char* d_stage = nullptr; int stage_bytes = 0;
+  float* terrain_origin = nullptr;   // caller-owned [n_envs, 2] terrain origin per env (locosim_set_terrain_origin), or NULL
   std::string err;
 };
 #ifndef LOCOSIM_EXTRA_CONFIGS_TU
@@ -1572,6 +1581,28 @@ extern "C" int locosim_configs31_forward(locosim_handle* h, const float* action,
 // __constant__ model slots (written at create and after a parameter-pool upload). Weak like the 31-dof entry points.
 extern "C" int locosim_ray_sync_model(locosim_handle* h) __attribute__((weak));
 extern "C" int locosim_ray_launch(locosim_handle* h, const RayArgs* a, cudaStream_t s) __attribute__((weak));
+// The terrain configuration (CfgEllEulerTerrain, index 6) is compiled in a fourth translation unit, locosim_terrain.cu, with
+// its own __constant__ slots (model, registered buffers, terrain), written by locosim_terrain_sync_model. Weak as well.
+extern "C" int locosim_terrain_setup(locosim_handle* h) __attribute__((weak));
+extern "C" int locosim_terrain_sync_model(locosim_handle* h) __attribute__((weak));
+extern "C" int locosim_terrain_step(locosim_handle* h, const float* a, float* o, float* r, uint8_t* d, float* no,
+                                    int auto_reset, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_terrain_body(locosim_handle* h, const uint8_t* mask, int parts, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_terrain_dataset_bodies(locosim_handle* h, float* body, float* next_body, cudaStream_t s)
+    __attribute__((weak));
+extern "C" int locosim_terrain_inverse(locosim_handle* h, const float* qacc, float* qfrc, cudaStream_t s)
+    __attribute__((weak));
+extern "C" int locosim_terrain_dataset_inverse(locosim_handle* h, float* qfrc, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_terrain_dynamics(locosim_handle* h, const DynOut* o, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_terrain_ray(locosim_handle* h, const RayArgs* a, cudaStream_t s) __attribute__((weak));
+extern "C" int locosim_terrain_forward(locosim_handle* h, const float* action, const FwdOut* o, cudaStream_t s)
+    __attribute__((weak));
+// the other translation units' copies of the handle's __constant__ slots (after a registration or a pool upload)
+static int sync_other_units(locosim_handle* h) {
+  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (h->cfg == 6 && locosim_terrain_sync_model(h)) return 1;
+  return 0;
+}
 
 // body_kernel outside a step, for the envs of `mask` (NULL = all), the parts (see body_kernel) that are registered:
 // d_next_body (1) after locosim_reset* and locosim_set_state; the reference keys (2) and d_next_ref (4) after locosim_reset*,
@@ -1586,6 +1617,7 @@ static int next_body_rows(locosim_handle* h, const uint8_t* mask, int parts, cud
     case 3: return launch_body<CfgPyrEuler29>(h, mask, nullptr, 0, parts, s);
     case 4:
     case 5: return locosim_configs31_body(h, mask, parts, s);
+    case 6: return locosim_terrain_body(h, mask, parts, s);
     default: return launch_body<CfgPyrRK4>(h, mask, nullptr, 0, parts, s);
   }
 }
@@ -1683,6 +1715,13 @@ int locosim_create(const int32_t* mi, int nmi, const double* mr, int nmr, const 
         h->err = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); rc = 1;
       }
       break;
+    case 6:
+      if (!locosim_terrain_setup) { h->err = "the terrain configuration is not compiled into this library"; rc = 1; break; }
+      rc = locosim_terrain_setup(h);
+      if (!rc && cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot) != cudaSuccess) {
+        h->err = std::string("cudaMemcpyToSymbol: ") + cudaGetErrorString(cudaGetLastError()); rc = 1;
+      }
+      break;
     default: rc = setup_cfg<CfgPyrRK4>(h); break;
   }
   if (!rc && locosim_ray_sync_model) rc = locosim_ray_sync_model(h);
@@ -1744,8 +1783,14 @@ int locosim_set_applied_forces(locosim_t* h, float* d_xfrc, float* d_qfrc) {
   h->applied.xfrc = d_xfrc; h->applied.qfrc = d_qfrc;
   // (the kernels read the pointers from the handle's __constant__ slot, in both translation units)
   CK(cudaMemcpyToSymbol(c_applied, &h->applied, sizeof(DevApplied), sizeof(DevApplied) * h->slot));
-  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (sync_other_units(h)) return 1;
   return 0;
+}
+int locosim_set_terrain_origin(locosim_t* h, float* d_origin) {
+  if (h->cfg != 6) { h->err = "this model has no terrain"; return 1; }
+  CK(cudaSetDevice(h->device));
+  h->terrain_origin = d_origin;
+  return locosim_terrain_sync_model(h);
 }
 int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body) {
   CK(cudaSetDevice(h->device));
@@ -1756,7 +1801,7 @@ int locosim_set_body_outputs(locosim_t* h, float* d_body, float* d_next_body) {
   h->bodyout.body = d_body; h->bodyout.next_body = d_next_body;
   // (a __constant__ table of its own in both translation units, like the applied forces)
   CK(cudaMemcpyToSymbol(c_bodyout, &h->bodyout, sizeof(DevBodyOut), sizeof(DevBodyOut) * h->slot));
-  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (sync_other_units(h)) return 1;
   return 0;
 }
 int locosim_set_reference_outputs(locosim_t* h, float* d_ref, float* d_next_ref) {
@@ -1766,7 +1811,7 @@ int locosim_set_reference_outputs(locosim_t* h, float* d_ref, float* d_next_ref)
   h->refout.ref = d_ref; h->refout.next_ref = d_next_ref; h->refout.key = on ? h->ref_key : nullptr;
   // (a __constant__ table of its own in both translation units, read by body_kernel when it runs)
   CK(cudaMemcpyToSymbol(c_refout, &h->refout, sizeof(DevRefOut), sizeof(DevRefOut) * h->slot));
-  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (sync_other_units(h)) return 1;
   if (!on) return 0;
   // every env's key from its current state (steps and resets keep them from here on); nothing else is written
   CK(cudaDeviceSynchronize());
@@ -1793,6 +1838,7 @@ int locosim_create_dataset_bodies(locosim_t* h, float* d_body, float* d_next_bod
     case 3: return launch_dataset_bodies<CfgPyrEuler29>(h, d_body, d_next_body, s);
     case 4:
     case 5: return locosim_configs31_dataset_bodies(h, d_body, d_next_body, s);
+    case 6: return locosim_terrain_dataset_bodies(h, d_body, d_next_body, s);
     default: return launch_dataset_bodies<CfgPyrRK4>(h, d_body, d_next_body, s);
   }
 }
@@ -1822,6 +1868,7 @@ int locosim_inverse(locosim_t* h, const float* d_qacc, float* d_qfrc_inverse, vo
     case 3: return launch_inverse<CfgPyrEuler29>(h, d_qacc, d_qfrc_inverse, s);
     case 4:
     case 5: return locosim_configs31_inverse(h, d_qacc, d_qfrc_inverse, s);
+    case 6: return locosim_terrain_inverse(h, d_qacc, d_qfrc_inverse, s);
     default: return launch_inverse<CfgPyrRK4>(h, d_qacc, d_qfrc_inverse, s);
   }
 }
@@ -1836,6 +1883,7 @@ int locosim_create_dataset_inverse(locosim_t* h, float* d_qfrc, void* stream) {
     case 3: return launch_dataset_inverse<CfgPyrEuler29>(h, d_qfrc, s);
     case 4:
     case 5: return locosim_configs31_dataset_inverse(h, d_qfrc, s);
+    case 6: return locosim_terrain_dataset_inverse(h, d_qfrc, s);
     default: return launch_dataset_inverse<CfgPyrRK4>(h, d_qfrc, s);
   }
 }
@@ -1856,6 +1904,7 @@ int locosim_dynamics_terms(locosim_t* h, float* d_M, float* d_bias, float* d_pas
     case 3: return launch_dynamics<CfgPyrEuler29>(h, o, s);
     case 4:
     case 5: return locosim_configs31_dynamics(h, &o, s);
+    case 6: return locosim_terrain_dynamics(h, &o, s);
     default: return launch_dynamics<CfgPyrRK4>(h, o, s);
   }
 }
@@ -1878,6 +1927,7 @@ int locosim_forward(locosim_t* h, const float* d_action, float* d_dof, float* d_
     case 3: return launch_forward<CfgPyrEuler29>(h, d_action, o, s);
     case 4:
     case 5: return locosim_configs31_forward(h, d_action, &o, s);
+    case 6: return locosim_terrain_forward(h, d_action, &o, s);
     default: return launch_forward<CfgPyrRK4>(h, d_action, o, s);
   }
 }
@@ -1902,6 +1952,7 @@ int locosim_ray(locosim_t* h, const float* d_pnt, const float* d_vec, int n_rays
   if (n == 0) return 0;
   CK(cudaSetDevice(h->device));
   const RayArgs a = {d_pnt, d_vec, d_dist, d_geom, d_normal, n_rays, frame, frame_body, exclude_body, flags};
+  if (h->cfg == 6) return locosim_terrain_ray(h, &a, (cudaStream_t)stream);
   return locosim_ray_launch(h, &a, (cudaStream_t)stream);
 }
 int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {
@@ -1911,7 +1962,7 @@ int locosim_set_contact_outputs(locosim_t* h, float* d_contact) {
   // (a __constant__ table of its own in both translation units; the step kernels read it when they run, so a step captured
   // in a CUDA graph before this call writes the buffer at its next replay)
   CK(cudaMemcpyToSymbol(c_contact, &h->contact, sizeof(DevContact), sizeof(DevContact) * h->slot));
-  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (sync_other_units(h)) return 1;
   return 0;
 }
 int locosim_set_dof_outputs(locosim_t* h, float* d_dof) {
@@ -1925,7 +1976,7 @@ int locosim_set_dof_outputs(locosim_t* h, float* d_dof) {
   h->dof.n_substeps = h->dt.n_substeps;
   // (__constant__ tables of their own in both translation units, read when the kernels run, as for the contact outputs)
   CK(cudaMemcpyToSymbol(c_dof, &h->dof, sizeof(DevDof), sizeof(DevDof) * h->slot));
-  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (sync_other_units(h)) return 1;
   return 0;
 }
 int locosim_max_contacts(const locosim_t* h) {
@@ -1935,6 +1986,7 @@ int locosim_max_contacts(const locosim_t* h) {
     case 3: return CfgPyrEuler29::MAXCON;
     case 4: return CfgPyrRK4_31::MAXCON;
     case 5: return CfgPyrEuler31::MAXCON;
+    case 6: return CfgEllEulerTerrain::MAXCON;
     default: return CfgPyrRK4::MAXCON;
   }
 }
@@ -1952,7 +2004,7 @@ int locosim_set_contact_list_outputs(locosim_t* h, int32_t* d_ncon, float* d_con
   // rows first, so that a kernel never sees the count pointer without them)
   CK(cudaMemcpyToSymbol(c_conrows, &h->conrows, sizeof(DevConRows), sizeof(DevConRows) * h->slot));
   CK(cudaMemcpyToSymbol(c_conlist, &h->conlist, sizeof(DevConList), sizeof(DevConList) * h->slot));
-  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (sync_other_units(h)) return 1;
   return 0;
 }
 int locosim_get_episode_stats(locosim_t* h, int32_t* d_len, float* d_ret, int32_t* d_last_len, float* d_last_ret, void* stream) {
@@ -2009,6 +2061,7 @@ int locosim_step(locosim_t* h, const float* a, float* o, float* r, uint8_t* d, f
     case 3: return launch_step<CfgPyrEuler29>(h, a, o, r, d, no, auto_reset, s);
     case 4:
     case 5: return locosim_configs31_step(h, a, o, r, d, no, auto_reset, s);
+    case 6: return locosim_terrain_step(h, a, o, r, d, no, auto_reset, s);
     default: return launch_step<CfgPyrRK4>(h, a, o, r, d, no, auto_reset, s);
   }
 }
@@ -2109,7 +2162,7 @@ int locosim_set_param_pool(locosim_t* h, const double* pool, int n_rows, int row
   h->dm.nfric = nfric;
   if (damp) h->dm.has_damping = 1;
   CK(cudaMemcpyToSymbol(c_models, &h->dm, sizeof(DevModel), sizeof(DevModel) * h->slot));
-  if ((h->cfg == 4 || h->cfg == 5) && locosim_configs31_sync_model(h)) return 1;
+  if (sync_other_units(h)) return 1;
   if (locosim_ray_sync_model && locosim_ray_sync_model(h)) return 1;
   CK(cudaMemset(h->st.dr_row, 0, (size_t)h->n_envs * 4));
   if (h->refout.key) {

@@ -209,6 +209,24 @@ __constant__ DevConRows c_conrows[LS_MAX_SLOTS];  // (likewise)
 __device__ unsigned long long g_dbg[8];      // (LOCOSIM_DEBUG & 8) MPR statistics: calls, support pairs, hits, cap exits
 #endif
 
+#ifdef LOCOSIM_TERRAIN
+// height field (terrain) of a handle, read by terrain_pass: only the translation unit of the terrain configuration
+// (locosim_terrain.cu) and the serial build define LOCOSIM_TERRAIN, so no other unit compiles any of this.
+// data: the ModelPack's hfield_data [nrow * ncol] (fp32, in the model's device copy); origin: the caller-owned [N, 2] terrain
+// origin per env (locosim_set_terrain_origin), row EnvS::env, NULL = zeros. The terrain pairs are pair_geom[p0, p0 + npair).
+struct DevTerrain {
+  const float* data;
+  const float* origin;
+  int nrow, ncol, geom, p0, npair;
+  float size[4], pos[3];
+};
+#ifdef LS_EMULATE
+static DevTerrain c_terrain[LS_MAX_SLOTS];
+#else
+__constant__ DevTerrain c_terrain[LS_MAX_SLOTS];
+#endif
+#endif
+
 // Phase clock: a diagnostic build (-DLOCOSIM_PHASE_CLOCK, tools/phase_profile.py) in which lane 0 of every warp adds the
 // clock64() cycles its env spends in each phase (or a count) to g_phase[slot][phase], one slot per (block mod 256, warp).
 // Without the macro the hooks expand to nothing, so the product library's code is the same as without them.
@@ -1474,6 +1492,7 @@ LS_DEV int box_box_edge(float margin, const float* p1, const float* m1, const fl
 //                                2 MPR ran, no contact; res[1..3] = the last direction tested (refreshes o's cache),
 //                                3 MPR ran, touching contact without a normal (ignored).
 #define LS_MAXJOB 32
+#define LS_MAXCONPAIR 50     // mjMAXCONPAIR: contacts of one pair (the terrain pass; every other routine returns at most 4)
 #define LS_CAND_HULL(pk) (((pk) >> 11) & 0x8000)     // pair flag 4 (bit 26 of pair_packed) as bit 15 of a candidate entry
 template <class C>
 LS_FN void convex_job(const int ms, const EnvS<C>& o, EnvS<C>& e, int p, float* res) {
@@ -1647,6 +1666,141 @@ LS_FN int pair_narrow(const int ms, EnvS<C>& e, int p, RawCon* raw, int* g1_out,
   *g1_out = g1; *g2_out = g2; *margin_out = margin;
   return n;
 }
+
+#ifdef LOCOSIM_TERRAIN
+// ---- mjc_ConvexHField: the pairs (terrain, g), after every other pair (include/locosim.h states the semantics) ----
+// Prism k of a cell range with nc columns: row r = k / (2 nc), column c, triangle tri = k % 2 (row, column, triangle order).
+// Its vertices (the strip order of MuJoCo's prism builder): triangle 0 = grid points (c, r), (c, r+1), (c+1, r); triangle
+// 1 = (c, r+1), (c+1, r), (c+1, r+1); the diagonal runs from (c+1, r) to (c, r+1). Vertex order: the three bottom points
+// (z = -base) first, then the three top points, each in that order (the support scan's first maximum wins: the same
+// vertex order in tests/csrc/terrain_ref.c).
+LS_DEV void terrain_prism(const DevTerrain& t, const int r, const int c, const int tri, float (*v)[3]) {
+  const int rr[3] = {tri ? r + 1 : r, tri ? r : r + 1, tri ? r + 1 : r};
+  const int c0[3] = {c, tri ? c + 1 : c, c + 1};
+  const float dx = 2.0f * t.size[0] / (float)(t.ncol - 1), dy = 2.0f * t.size[1] / (float)(t.nrow - 1);
+  for (int i = 0; i < 3; i++) {
+    const float x = dx * (float)c0[i] - t.size[0], y = dy * (float)rr[i] - t.size[1];
+    v[i][0] = v[3 + i][0] = x;
+    v[i][1] = v[3 + i][1] = y;
+    v[i][2] = -t.size[3];
+    v[3 + i][2] = LS_LDG(t.data + rr[i] * t.ncol + c0[i]) * t.size[2];
+  }
+}
+// half extent of a geom's support along the unit axis k of its frame's parent (closed form for sphere / capsule / cylinder
+// / box, all symmetric about their centre)
+LS_DEV float terrain_extent(const int type, const float* mat, const float* size, const int k) {
+  const float a = fabsf(mat[3 * k + 2]);
+  if (type == LS_GEOM_SPHERE) return size[0];
+  if (type == LS_GEOM_CAPSULE) return size[0] + size[1] * a;
+  if (type == LS_GEOM_CYLINDER) return size[0] * sqrtf(fmaxf(1.0f - a * a, 0.0f)) + size[1] * a;
+  return fabsf(mat[3 * k]) * size[0] + fabsf(mat[3 * k + 1]) * size[1] + a * size[2];
+}
+template <class C>
+LS_FN void terrain_pass(const int ms, EnvS<C>& e) {
+  const DevModel& m = c_models[ms];
+  const DevTerrain& t = c_terrain[ms];
+  constexpr int SCR = (int)((sizeof(MprScratch) + 15) / 16 * 4);
+  MprScratch* sc = reinterpret_cast<MprScratch*>(&e.J[0][0]);      // (convex_job's scratch: free until make_constraint)
+  float* buf = &e.J[0][0] + SCR;
+  // the field's frame in the world: its geom position moved by -origin[env]
+  float f[3] = {t.pos[0], t.pos[1], t.pos[2]};
+  // (e.env < 0: a dataset row of locosim_create_dataset_inverse, which is not an env: the zero origin)
+  if (t.origin && e.env >= 0) { f[0] -= LS_LDG(t.origin + 2 * e.env); f[1] -= LS_LDG(t.origin + 2 * e.env + 1); }
+  const float dx = 2.0f * t.size[0] / (float)(t.ncol - 1), dy = 2.0f * t.size[1] / (float)(t.nrow - 1);
+  NOUNROLL for (int q = 0; q < t.npair; q++) {
+    if (e.ncon >= EnvS<C>::MAXCON) break;
+    const int g1 = t.geom, g2 = m.pair_geom[2 * (t.p0 + q) + 1];
+    const int t2 = m.geom_type[g2];
+    const float margin = fmaxf(m.geom_margin[g1], m.geom_margin[g2]);
+    float mat[9];
+    geom_mat(ms, e, g2, mat);
+    const float* sz = m.geom_size + 3 * g2;
+    const float p[3] = {e.gxpos[g2][0] - f[0], e.gxpos[g2][1] - f[1], e.gxpos[g2][2] - f[2]};
+    if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]))) continue;      // (no cell range for a non-finite pose)
+    const float hx = terrain_extent(t2, mat, sz, 0), hy = terrain_extent(t2, mat, sz, 1), hz = terrain_extent(t2, mat, sz, 2);
+    const float zmin = p[2] - hz;
+    if (p[0] - hx - margin > t.size[0] || p[0] + hx + margin < -t.size[0] || p[1] - hy - margin > t.size[1] ||
+        p[1] + hy + margin < -t.size[1] || zmin - margin > t.size[2] || p[2] + hz + margin < -t.size[3])
+      continue;
+    // cell range of the box (floor / ceil of the grid coordinates, clamped to the grid)
+    int cmin = (int)floorf((p[0] - hx - margin + t.size[0]) / dx), cmax = (int)ceilf((p[0] + hx + margin + t.size[0]) / dx);
+    int rmin = (int)floorf((p[1] - hy - margin + t.size[1]) / dy), rmax = (int)ceilf((p[1] + hy + margin + t.size[1]) / dy);
+    cmin = cmin < 0 ? 0 : cmin; rmin = rmin < 0 ? 0 : rmin;
+    cmax = cmax > t.ncol - 1 ? t.ncol - 1 : cmax; rmax = rmax > t.nrow - 1 ? t.nrow - 1 : rmax;
+    const int nc = cmax - cmin, nprism = 2 * nc * (rmax - rmin);
+    const float incl = pair_incl(m, g1, g2, margin);
+    int cnt = 0;
+    NOUNROLL for (int base = 0; base < nprism && cnt < LS_MAXCONPAIR; base += 32) {
+      // the lanes test 32 prisms at once (all three top points below the geom's lowest point: skipped), the warp then runs
+      // MPR on the rest in order
+#ifdef LS_EMULATE
+      unsigned live = 0;
+      for (int l = 0; l < 32 && base + l < nprism; l++) {
+        const int k = base + l, r = rmin + k / (2 * nc), c = cmin + (k % (2 * nc)) / 2;
+        float v[6][3];
+        terrain_prism(t, r, c, k & 1, v);
+        if (!(v[3][2] < zmin - margin && v[4][2] < zmin - margin && v[5][2] < zmin - margin)) live |= 1u << l;
+      }
+#else
+      bool ok = false;
+      {
+        const int k = base + LS_LANE;
+        if (k < nprism) {
+          const int r = rmin + k / (2 * nc), c = cmin + (k % (2 * nc)) / 2;
+          float v[6][3];
+          terrain_prism(t, r, c, k & 1, v);
+          ok = !(v[3][2] < zmin - margin && v[4][2] < zmin - margin && v[5][2] < zmin - margin);
+        }
+      }
+      unsigned live = __ballot_sync(0xffffffffu, ok);
+#endif
+      while (live && cnt < LS_MAXCONPAIR && e.ncon < EnvS<C>::MAXCON) {
+        const int l = LS_FFS(live) - 1;
+        live &= live - 1;
+        const int k = base + l, r = rmin + k / (2 * nc), c = cmin + (k % (2 * nc)) / 2;
+        LANE0 {
+          float v[6][3], cen[3] = {0, 0, 0};
+          terrain_prism(t, r, c, k & 1, v);
+          for (int i = 0; i < 6; i++)
+            for (int j = 0; j < 3; j++) { buf[3 * i + j] = v[i][j] + f[j]; cen[j] += v[i][j]; }
+          MprGeom& a = sc->g[0];
+          MprGeom& b = sc->g[1];
+          a.type = LS_GEOM_MESH; a.vnum = 6; a.world = 1; a.verts = buf; a.margin = 0.5f * margin;
+          b.type = t2; b.vnum = 0; b.world = 0; b.verts = nullptr; b.margin = 0.5f * margin;
+          for (int j = 0; j < 3; j++) {
+            a.pos[j] = cen[j] * (1.0f / 6.0f) + f[j];
+            b.pos[j] = e.gxpos[g2][j];
+            b.size[j] = sz[j];
+          }
+          for (int j = 0; j < 9; j++) b.mat[j] = mat[j];
+        }
+        SYNC();
+        float depth, dir[3], pos[3], sep[3];
+        const bool hit = mpr_penetration(sc, &depth, dir, pos, sep);
+        SYNC();
+        LANE0 { e.mpr_calls += 1; }
+#if defined(LS_EMULATE)
+        g_mpr_calls++;
+#endif
+        if (hit && !(dir[0] == 0.0f && dir[1] == 0.0f && dir[2] == 0.0f)) {
+          cnt++;
+          const float dist = margin - depth;
+          if (dist < incl) {
+            LANE0 {
+              RawCon rc;
+              rc.dist = dist;
+              for (int j = 0; j < 3; j++) { rc.pos[j] = pos[j]; rc.frame[j] = dir[j]; rc.frame[3 + j] = 0; }
+              fill_contact(ms, e, e.ncon, g1, g2, incl, &rc);
+              e.ncon = e.ncon + 1;
+            }
+            SYNC();
+          }
+        }
+      }
+    }
+  }
+}
+#endif
 
 template <class C>
 LS_FN void collision(const int ms, EnvS<C>& e) {
@@ -1881,6 +2035,9 @@ LS_FN void collision(const int ms, EnvS<C>& e) {
     }
     PH_LAP(PH_COL_CONSUME, tc);
   }
+#endif
+#ifdef LOCOSIM_TERRAIN
+  if constexpr (C::TERRAIN) { SYNC(); terrain_pass(ms, e); }
 #endif
   SYNC();
 }
@@ -4014,3 +4171,113 @@ LS_DEV float ray_geoms(const RayGeom* G, const int ng, const float* p, const flo
   *geom = bg;
   return best;
 }
+
+#ifdef LOCOSIM_TERRAIN
+// ---- mj_rayHfield: a ray against the terrain solid of env `env` (include/locosim.h: the top surface's triangles with the
+// collision's diagonal, the four sides and the base at -base). In the field's frame (unrotated: a translation by the
+// field's position moved by -origin[env]); returns the first hit in units of |v| (-1: none) and the outward unit normal.
+// The top surface is walked cell by cell along the ray (2D DDA between the ray's entry into and exit from the field's
+// box); the triangles are intersected two-sided (Moeller-Trumbore), the sides and the base as bounded planes.
+LS_DEV float ray_tri(const float* o, const float* v, const float* a, const float* b, const float* c, float* n) {
+  const float e1[3] = {b[0] - a[0], b[1] - a[1], b[2] - a[2]}, e2[3] = {c[0] - a[0], c[1] - a[1], c[2] - a[2]};
+  float h[3], q[3];
+  cross3(h, v, e2);
+  const float det = dot3(e1, h);
+  if (fabsf(det) < 1e-20f) return -1;
+  const float inv = 1.0f / det, s[3] = {o[0] - a[0], o[1] - a[1], o[2] - a[2]};
+  const float u = inv * dot3(s, h);
+  if (u < 0 || u > 1) return -1;
+  cross3(q, s, e1);
+  const float w = inv * dot3(v, q);
+  if (w < 0 || u + w > 1) return -1;
+  const float x = inv * dot3(e2, q);
+  if (x < 0) return -1;
+  cross3(n, e1, e2);
+  if (n[2] < 0) { n[0] = -n[0]; n[1] = -n[1]; n[2] = -n[2]; }
+  return x;
+}
+LS_DEV float ray_hfield(const DevTerrain& t, const float* lp, const float* v, float* n) {
+  const float rx = t.size[0], ry = t.size[1], el = t.size[2], bs = t.size[3];
+  const float lo[3] = {-rx, -ry, -bs}, hi[3] = {rx, ry, el};
+  float tin = 0.0f, tout = 3.0e38f;
+  for (int k = 0; k < 3; k++) {
+    if (fabsf(v[k]) < LS_MINVAL) { if (lp[k] < lo[k] || lp[k] > hi[k]) return -1; continue; }
+    const float a = (lo[k] - lp[k]) / v[k], b = (hi[k] - lp[k]) / v[k];
+    tin = fmaxf(tin, fminf(a, b)); tout = fminf(tout, fmaxf(a, b));
+  }
+  if (tin > tout) return -1;
+  const int nr = t.nrow, nc = t.ncol;
+  const float dx = 2.0f * rx / (float)(nc - 1), dy = 2.0f * ry / (float)(nr - 1);
+  float best = -1;
+  auto clampi = [](int x, int a, int b) { return x < a ? a : (x > b ? b : x); };
+  auto take = [&](float x, const float* nn) {
+    if (x >= 0 && (best < 0 || x < best)) { best = x; n[0] = nn[0]; n[1] = nn[1]; n[2] = nn[2]; }
+  };
+  // sides (x = -+rx: column 0 / ncol - 1; y = -+ry: row 0 / nrow - 1) up to the surface height along the edge, and the base
+  for (int sd = 0; sd < 4; sd++) {
+    const int ax = sd >> 1, oth = 1 - ax;
+    const float plane = (sd & 1) ? hi[ax] : lo[ax];
+    if (fabsf(v[ax]) < LS_MINVAL) continue;
+    const float x = (plane - lp[ax]) / v[ax];
+    if (x < 0) continue;
+    const float w = lp[oth] + x * v[oth], z = lp[2] + x * v[2];
+    if (w < lo[oth] || w > hi[oth] || z < -bs) continue;
+    const int ns = ax ? nc : nr;                           // samples along the edge
+    const float ds = ax ? dx : dy, g = (w - lo[oth]) / ds;
+    const int i = clampi((int)floorf(g), 0, ns - 2);
+    const int fixed = (sd & 1) ? (ax ? nr - 1 : nc - 1) : 0;
+    const int i0 = ax ? fixed * nc + i : i * nc + fixed, i1 = ax ? i0 + 1 : i0 + nc;
+    const float f = g - (float)i, hz = (LS_LDG(t.data + i0) * (1.0f - f) + LS_LDG(t.data + i1) * f) * el;
+    if (z > hz) continue;
+    float nn[3] = {0, 0, 0};
+    nn[ax] = (sd & 1) ? 1.0f : -1.0f;
+    take(x, nn);
+  }
+  if (fabsf(v[2]) >= LS_MINVAL) {
+    const float x = (-bs - lp[2]) / v[2], px = lp[0] + x * v[0], py = lp[1] + x * v[1];
+    const float nn[3] = {0, 0, -1};
+    if (x >= 0 && px >= -rx && px <= rx && py >= -ry && py <= ry) take(x, nn);
+  }
+  // the top surface, cell by cell from the ray's entry into the box
+  const float x0 = lp[0] + tin * v[0], y0 = lp[1] + tin * v[1];
+  int c = clampi((int)floorf((x0 + rx) / dx), 0, nc - 2), r = clampi((int)floorf((y0 + ry) / dy), 0, nr - 2);
+  const int sc = v[0] > 0 ? 1 : -1, sr = v[1] > 0 ? 1 : -1;
+  const float tdx = fabsf(v[0]) > LS_MINVAL ? dx / fabsf(v[0]) : 3.0e38f, tdy = fabsf(v[1]) > LS_MINVAL ? dy / fabsf(v[1]) : 3.0e38f;
+  float tnx = fabsf(v[0]) > LS_MINVAL ? ((float)(c + (sc > 0)) * dx - rx - lp[0]) / v[0] : 3.0e38f;
+  float tny = fabsf(v[1]) > LS_MINVAL ? ((float)(r + (sr > 0)) * dy - ry - lp[1]) / v[1] : 3.0e38f;
+  for (int guard = 0; guard < nr + nc; guard++) {
+    for (int tri = 0; tri < 2; tri++) {
+      const int rr[3] = {tri ? r + 1 : r, tri ? r : r + 1, tri ? r + 1 : r};
+      const int cc[3] = {c, tri ? c + 1 : c, c + 1};
+      float P[3][3], nn[3];
+      for (int i = 0; i < 3; i++) {
+        P[i][0] = dx * (float)cc[i] - rx; P[i][1] = dy * (float)rr[i] - ry;
+        P[i][2] = LS_LDG(t.data + rr[i] * nc + cc[i]) * el;
+      }
+      const float x = ray_tri(lp, v, P[0], P[1], P[2], nn);
+      if (x >= 0) { const float il = rsqrtf(dot3(nn, nn)); nn[0] *= il; nn[1] *= il; nn[2] *= il; take(x, nn); }
+    }
+    const float tnext = fminf(tnx, tny);
+    if ((best >= 0 && best <= tnext) || tnext > tout) break;     // (a later cell's hits lie beyond this cell's exit)
+    if (tnx < tny) { c += sc; tnx += tdx; } else { r += sr; tny += tdy; }
+    if (c < 0 || c > nc - 2 || r < 0 || r > nr - 2) break;
+  }
+  return best;
+}
+// the terrain's hit of a ray of env `env` (world frame), merged into the nearest hit of the other geoms (dist / geom / nrm,
+// as ray_geoms returns them): the terrain is welded to the world (LS_RAY_STATIC, body 0)
+LS_DEV void ray_terrain(const int ms, const int env, const float* p, const float* v, const int exclude, const int sel,
+                        float* dist, int* geom, float* nrm) {
+  const DevTerrain& t = c_terrain[ms];
+  if (!(sel & LS_RAY_STATIC) || exclude == 0 || !(dot3(v, v) > 0)) return;
+  float f[3] = {t.pos[0], t.pos[1], t.pos[2]};
+  if (t.origin) { f[0] -= LS_LDG(t.origin + 2 * env); f[1] -= LS_LDG(t.origin + 2 * env + 1); }
+  const float lp[3] = {p[0] - f[0], p[1] - f[1], p[2] - f[2]};
+  float n[3];
+  const float x = ray_hfield(t, lp, v, n);
+  if (x >= 0 && (*dist < 0 || x < *dist)) {
+    *dist = x; *geom = t.geom;
+    for (int k = 0; k < 3; k++) nrm[k] = n[k];
+  }
+}
+#endif

@@ -1,6 +1,7 @@
 // Serial CPU emulation of the warp-cooperative engine core (development aid only; see locosim_core.cuh).
 // Built by tools/build_emu.sh into scratch/; NOT shipped, NOT loaded by the product path.
 #define LS_EMULATE 1
+#define LOCOSIM_TERRAIN 1      // (the terrain configuration's collision pass: see locosim_terrain.cu)
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -16,6 +17,7 @@ struct EmuBase {
   DevDof dof = {nullptr, 1};
   DevConList cl = {nullptr, 1};
   DevConRows cr = {nullptr, nullptr};
+  DevTerrain terr = {};              // the terrain configuration's height field; origin: row 0 of the engine's [N, 2]
   std::vector<float> act;            // the dof outputs' actuator-force scratch (row 0 of the engine's [N, nu])
   SolverOpts so;
   std::vector<int> grf_group; int n_grf = 0;
@@ -49,7 +51,7 @@ struct EmuT : EmuBase {
   }
   void step(const double* ctrl, int nsub) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
-    c_models[0] = m; c_applied[0] = ap; c_contact[0] = cw; c_contact[0].n_substeps = nsub;
+    c_models[0] = m; c_terrain[0] = terr; c_applied[0] = ap; c_contact[0] = cw; c_contact[0].n_substeps = nsub;
     c_dof[0] = dof; c_dof[0].n_substeps = nsub; c_dof_act[0] = dof.out ? act.data() : nullptr;
     c_conlist[0] = cl; c_conlist[0].n_substeps = nsub; c_conrows[0] = cr;
     e.substep = 0;
@@ -57,7 +59,7 @@ struct EmuT : EmuBase {
   }
   void fwd(const double* ctrl) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
-    c_models[0] = m; c_applied[0] = ap; c_dof[0] = dof; c_dof_act[0] = dof.out ? act.data() : nullptr;
+    c_models[0] = m; c_terrain[0] = terr; c_applied[0] = ap; c_dof[0] = dof; c_dof_act[0] = dof.out ? act.data() : nullptr;
     forward(0, e, so);
   }
   void get(double* q, double* v, double* qacc, double* ws) override {
@@ -100,25 +102,25 @@ struct EmuT : EmuBase {
     for (int k = 0; k < 3 * LS_MAX_GRF; k++) e.grf[k] = keep->grf[k];
     delete keep;
   }
-  void body(float* out) override { c_models[0] = m; body_outputs(0, e, out, (float*)nullptr); }
+  void body(float* out) override { c_models[0] = m; c_terrain[0] = terr; body_outputs(0, e, out, (float*)nullptr); }
   void ref(const DevTask& t, const float* row, float angle, float* out) override {
-    c_models[0] = m;
+    c_models[0] = m; c_terrain[0] = terr;
     reference_outputs(0, t, e, row, angle, out, (float*)nullptr);
   }
   void inv(const double* qacc, float* out) override {
-    c_models[0] = m;
+    c_models[0] = m; c_terrain[0] = terr;
     e.substep = -1;
     for (int i = 0; i < m.nv; i++) e.qacc[i] = (float)qacc[i];
     inverse_dynamics(0, e, out);
   }
   void dyn(const DynOut& o) override {
-    c_models[0] = m;
+    c_models[0] = m; c_terrain[0] = terr;
     e.substep = -1;
     dynamics_terms(0, e, o);
   }
   void fwd_out(const double* ctrl, const FwdOut& o) override {
     for (int i = 0; i < m.nu; i++) e.ctrl[i] = (float)ctrl[i];
-    c_models[0] = m; c_applied[0] = ap;
+    c_models[0] = m; c_terrain[0] = terr; c_applied[0] = ap;
     e.substep = -1;
     init_workspace(0, e);
     forward_dynamics(0, e, so, o);
@@ -126,7 +128,7 @@ struct EmuT : EmuBase {
   int max_contacts() override { return C::MAXCON; }
   void ray(const float* pnt, const float* vec, int n_rays, int frame, int fb, int exclude, int flags, float* dist, int* geom,
            float* normal) override {
-    c_models[0] = m;
+    c_models[0] = m; c_terrain[0] = terr;
     const bool bad = nonfinite_state(e, m.nv);
     std::vector<RayGeom> G(m.ng);
     if (!bad) {
@@ -139,11 +141,12 @@ struct EmuT : EmuBase {
       if (!bad) {
         ray_to_world(e, frame, fb, pnt + 3 * k, vec + 3 * k, p, v);
         dist[k] = ray_geoms(G.data(), m.ng, p, v, exclude, flags, geom + k, nrm);
+        if (C::TERRAIN) ray_terrain(0, 0, p, v, exclude, flags, dist + k, geom + k, nrm);
       }
       if (normal) for (int c = 0; c < 3; c++) normal[3 * k + c] = nrm[c];
     }
   }
-  void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; init_workspace(0, e); }
+  void bind_prm() override { e.prm = hm.default_row.data(); e.pk_tab = m.pair_packed; c_models[0] = m; c_terrain[0] = terr; init_workspace(0, e); }
 };
 
 extern "C" {
@@ -165,10 +168,18 @@ EmuBase* emu_create(const int* ints, int n_ints, const double* reals, int n_real
     case 3: s = new EmuT<CfgPyrEuler29>(); break;
     case 4: s = new EmuT<CfgPyrRK4_31>(); break;
     case 5: s = new EmuT<CfgPyrEuler31>(); break;
+    case 6: s = new EmuT<CfgEllEulerTerrain>(); break;
     default: fprintf(stderr, "emu: no compiled configuration fits this model\n"); return nullptr;
   }
   s->hm = hm;
   bind_model(s->m, s->hm, s->hm.ints.data(), s->hm.reals.data());
+  if (s->hm.hf_nrow > 0) {
+    DevTerrain& t = s->terr;
+    t.data = s->hm.reals.data() + s->hm.hf_off; t.origin = nullptr;
+    t.nrow = s->hm.hf_nrow; t.ncol = s->hm.hf_ncol; t.geom = s->hm.hf_geom; t.p0 = s->hm.np - s->hm.nterr; t.npair = s->hm.nterr;
+    for (int k = 0; k < 4; k++) t.size[k] = s->hm.hf_size[k];
+    for (int k = 0; k < 3; k++) t.pos[k] = s->hm.hf_pos[k];
+  }
   s->bind_prm();
   s->so.tolerance = 1e-5f; s->so.ls_tolerance = 0.1f; s->so.max_iter = 20; s->so.ls_iter = 16;
   return s;
@@ -240,6 +251,9 @@ void emu_ray(EmuBase* s, const float* pnt, const float* vec, int n_rays, int fra
              float* dist, int* geom, float* normal) {
   s->ray(pnt, vec, n_rays, frame, fb, exclude, flags, dist, geom, normal);
 }
+// terrain origin of the emulated env (locosim_set_terrain_origin; row 0 of the engine's layout: fp32 [2], or NULL = zeros),
+// read by every later step and query from the caller's memory
+void emu_set_terrain_origin(EmuBase* s, float* origin) { s->terr.origin = origin; }
 // the configuration's per-env contact cap (locosim_max_contacts)
 int emu_max_contacts(EmuBase* s) { return s->max_contacts(); }
 long emu_mpr_stat(int k) { long v[8] = {g_forward_evals, g_mpr_candidates, g_mpr_calls, g_mpr_supports, g_sep_found, g_sep_ok, g_mpr_nohit, g_obb_pass}; return v[k]; }
@@ -268,6 +282,7 @@ int emu_sizeof_env(int which) {
     case 3: return (int)sizeof(EnvS<CfgPyrEuler29>);
     case 4: return (int)sizeof(EnvS<CfgPyrRK4_31>);
     case 5: return (int)sizeof(EnvS<CfgPyrEuler31>);
+    case 6: return (int)sizeof(EnvS<CfgEllEulerTerrain>);
     default: return (int)sizeof(EnvS<CfgPyrRK4>);
   }
 }

@@ -16,6 +16,11 @@ struct HostModel {
   float timestep, gravity[3], impratio, tolerance, meaninertia;
   int max_condim;
   int np_prim;                 // leading primitive pairs of the candidate-pair table (the general convex pairs follow)
+  int nterr = 0;               // trailing pairs (terrain, g) of the table; the mid-phase tables cover the np - nterr others
+  int hf_nrow = 0, hf_ncol = 0, hf_geom = -1;   // height field (terrain) grid and geom; hf_nrow = 0: no terrain
+  float hf_size[4] = {0, 0, 0, 0};              // (rx, ry, elevation, base)
+  float hf_pos[3] = {0, 0, 0};                  // the terrain geom's position (its frame's origin in the world)
+  size_t hf_off = 0;           // offset of hfield_data[nrow * ncol] in `reals` (after the wire fields)
   int po[13], pool_P;          // parameter pool row layout (float offsets), see domain_randomization.py POOL_FIELDS
   std::vector<float> default_row;   // the model's own parameters as one pool row
 };
@@ -38,10 +43,17 @@ static inline std::string parse_model(HostModel& h, const int* ints, int n_ints,
 #define X(name, cnt) nr += (size_t)(cnt);
   LOCOSIM_MP_REAL_FIELDS(X)
 #undef X
-  if ((size_t)n_ints != MPI_HEADER_LEN + ni || (size_t)n_reals != MPR_HEADER_LEN + nr) return "ModelPack size mismatch";
+  h.hf_nrow = ints[MPI_HF_NROW]; h.hf_ncol = ints[MPI_HF_NCOL];
+  if (h.hf_nrow < 0 || h.hf_ncol < 0 || (h.hf_nrow > 0) != (h.hf_ncol > 0) || (h.hf_nrow > 0 && (h.hf_nrow < 2 || h.hf_ncol < 2)))
+    return "bad height field grid (nrow, ncol >= 2, or both 0)";
+  if ((size_t)h.hf_nrow * (size_t)h.hf_ncol > (1u << 24)) return "height field larger than 2^24 samples";
+  const size_t nhf = (size_t)h.hf_nrow * (size_t)h.hf_ncol;
+  for (int k = 0; k < 4; k++) h.hf_size[k] = (float)reals[MPR_HF_SIZE + k];
+  if ((size_t)n_ints != MPI_HEADER_LEN + ni || (size_t)n_reals != MPR_HEADER_LEN + nr + nhf) return "ModelPack size mismatch";
   h.ints.assign(ints + MPI_HEADER_LEN, ints + n_ints);
-  h.reals.resize(nr);
-  for (size_t i = 0; i < nr; i++) h.reals[i] = (float)reals[MPR_HEADER_LEN + i];
+  h.reals.resize(nr + nhf);
+  for (size_t i = 0; i < nr + nhf; i++) h.reals[i] = (float)reals[MPR_HEADER_LEN + i];
+  h.hf_off = nr;
   // locate the arrays we need for the derived tables
   const int* ip = h.ints.data();
   const int *body_parentid = 0, *body_lastdof = 0, *dof_parentid = 0, *geom_condim = 0, *pair_geom = 0, *geom_type = 0;
@@ -55,10 +67,12 @@ static inline std::string parse_model(HostModel& h, const int* ints, int n_ints,
   LOCOSIM_MP_INT_FIELDS(X)
 #undef X
   const float* rp = h.reals.data();
-  const float *dof_frictionloss = 0, *dof_damping = 0, *geom_rbound = 0;
+  const float *dof_frictionloss = 0, *dof_damping = 0, *geom_rbound = 0, *geom_quat = 0, *geom_pos = 0;
 #define X(name, cnt) if (std::string(#name) == "dof_frictionloss") dof_frictionloss = rp; \
                      if (std::string(#name) == "dof_damping") dof_damping = rp;           \
                      if (std::string(#name) == "geom_rbound") geom_rbound = rp;           \
+                     if (std::string(#name) == "geom_quat") geom_quat = rp;               \
+                     if (std::string(#name) == "geom_pos") geom_pos = rp;                 \
                      rp += (cnt);
   LOCOSIM_MP_REAL_FIELDS(X)
 #undef X
@@ -90,6 +104,26 @@ static inline std::string parse_model(HostModel& h, const int* ints, int n_ints,
   // rbound[g1] + rbound[g2])
   if (ng >= 4096) return "more than 4095 geoms";
   if (np >= 32768) return "more than 32767 candidate pairs";         // (15-bit pair index in collision()'s candidate list)
+  // the terrain: the last geom, on the world body, unrotated; its pairs (terrain, g) close the pair table
+  {
+    int nhfg = 0;
+    for (int g = 0; g < ng; g++) if (geom_type[g] == LS_GEOM_HFIELD) nhfg++;
+    if (nhfg != (h.hf_nrow > 0 ? 1 : 0) || (nhfg && geom_type[ng - 1] != LS_GEOM_HFIELD))
+      return "a height field needs its grid, and is the model's last geom (one per model)";
+    if (nhfg) {
+      h.hf_geom = ng - 1;
+      const float* q = geom_quat + 4 * (ng - 1);
+      if (!(q[0] == 1.0f && q[1] == 0.0f && q[2] == 0.0f && q[3] == 0.0f)) return "a rotated height field is not supported";
+      if (!(h.hf_size[0] > 0 && h.hf_size[1] > 0 && h.hf_size[2] >= 0 && h.hf_size[3] > 0)) return "bad height field size";
+      for (int k = 0; k < 3; k++) h.hf_pos[k] = geom_pos[3 * (ng - 1) + k];
+    }
+    int nt = 0;
+    while (nt < np && geom_type[pair_geom[2 * (np - 1 - nt)]] == LS_GEOM_HFIELD) nt++;
+    for (int p = 0; p < np - nt; p++)
+      if (geom_type[pair_geom[2 * p]] == LS_GEOM_HFIELD) return "terrain pairs not last in the candidate-pair table (modelpack.pack)";
+    h.nterr = nt;
+    np -= nt;                                    // (the mid-phase tables below cover the other pairs)
+  }
   h.np_prim = np;
   bool seen_convex = false;
   for (int p = 0; p < np; p++) {
@@ -153,7 +187,8 @@ static inline void bind_model(DevModel& m, const HostModel& h, const int* ibase,
   m.integrator = h.integrator; m.cone = h.cone; m.iterations = h.iterations; m.nlevel = h.nlevel; m.nfric = h.nfric;
   m.timestep = h.timestep; m.gravity[0] = h.gravity[0]; m.gravity[1] = h.gravity[1]; m.gravity[2] = h.gravity[2];
   m.impratio = h.impratio; m.tolerance = h.tolerance; m.meaninertia = h.meaninertia; m.has_damping = h.has_damping;
-  m.np_prim = h.np_prim; m.pk_n = h.np;
+  m.np_prim = h.np_prim; m.pk_n = h.np - h.nterr;
+  m.np = h.np - h.nterr;           // (the terrain pairs are the terrain pass's: locosim_core.cuh terrain_pass)
   const int nb = h.nb, nv = h.nv, ng = h.ng, nu = h.nu, np = h.np, nm = h.nm;
   const int* ip = ibase;
   const float* rp = rbase;
@@ -167,8 +202,8 @@ static inline void bind_model(DevModel& m, const HostModel& h, const int* ibase,
   m.body_dofmask = ip; ip += nb;
   m.dof_frow = ip; ip += nv;
   m.tri_ij = ip; ip += 32 * 33 / 2;
-  m.pair_packed = ip; ip += np;
-  m.pair_bound = reinterpret_cast<const float*>(ip); ip += np;
+  m.pair_packed = ip; ip += m.np;
+  m.pair_bound = reinterpret_cast<const float*>(ip); ip += m.np;
   m.po_dof_damping = h.po[0]; m.po_dof_frictionloss = h.po[1]; m.po_dof_armature = h.po[2]; m.po_jnt_stiffness = h.po[3];
   m.po_dof_invweight0 = h.po[4]; m.po_body_mass = h.po[5]; m.po_body_inertia = h.po[6]; m.po_body_ipos = h.po[7];
   m.po_body_iquat = h.po[8]; m.po_geom_friction = h.po[9]; m.po_geom_invweight0 = h.po[10]; m.po_meaninertia = h.po[11]; m.po_user = h.po[12];
@@ -180,14 +215,14 @@ static inline void bind_model(DevModel& m, const HostModel& h, const int* ibase,
 static inline bool has_convex_pairs(const HostModel& hm) {
   DevModel v;
   bind_model(v, hm, hm.ints.data(), hm.reals.data());
-  for (int p = 0; p < hm.np; p++)
+  for (int p = 0; p < v.np; p++)
     if (v.pair_packed[p] & (2 << 24)) return true;
   return false;
 }
 static inline bool has_boxbox_pairs(const HostModel& hm) {
   DevModel v;
   bind_model(v, hm, hm.ints.data(), hm.reals.data());
-  for (int p = 0; p < hm.np; p++)
+  for (int p = 0; p < v.np; p++)
     if (v.geom_type[v.pair_geom[2 * p]] == LS_GEOM_BOX && v.geom_type[v.pair_geom[2 * p + 1]] == LS_GEOM_BOX) return true;
   return false;
 }
@@ -195,12 +230,15 @@ template <class C>
 static inline bool cfg_fits(const HostModel& hm, int obs_dim) {
   if (!C::CONVEX && has_convex_pairs(hm)) return false;
   if (!C::BOXBOX && has_boxbox_pairs(hm)) return false;
+  if ((int)C::TERRAIN != (hm.hf_nrow > 0 ? 1 : 0)) return false;
   return hm.nv <= C::NV && hm.nb <= C::NB && hm.ng <= C::NG && obs_dim <= C::MAXOBS && hm.cone == (int)C::CONE &&
          hm.integrator == (int)C::RK4;
 }
-// 0 CfgEllEuler, 1 CfgPyrEuler, 2 CfgPyrRK4, 3 CfgPyrEuler29, 4 CfgPyrRK4_31, 5 CfgPyrEuler31, -1 none fits (the first
-// that fits wins, so a model keeps the smallest configuration it fits)
+// 0 CfgEllEuler, 1 CfgPyrEuler, 2 CfgPyrRK4, 3 CfgPyrEuler29, 4 CfgPyrRK4_31, 5 CfgPyrEuler31, 6 CfgEllEulerTerrain, -1 none
+// fits (the first that fits wins, so a model keeps the smallest configuration it fits; a model with a terrain fits
+// CfgEllEulerTerrain only)
 static inline int select_cfg(const HostModel& hm, int obs_dim) {
+  if (hm.hf_nrow > 0) return cfg_fits<CfgEllEulerTerrain>(hm, obs_dim) ? 6 : -1;
   if (cfg_fits<CfgEllEuler>(hm, obs_dim)) return 0;
   if (cfg_fits<CfgPyrEuler>(hm, obs_dim)) return 1;
   if (cfg_fits<CfgPyrRK4>(hm, obs_dim)) return 2;

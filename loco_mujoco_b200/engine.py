@@ -83,6 +83,8 @@ def load_library():
     lib.locosim_nbody.argtypes = [vp]
     lib.locosim_set_applied_forces.restype = ip
     lib.locosim_set_applied_forces.argtypes = [vp, vp, vp]
+    lib.locosim_set_terrain_origin.restype = ip
+    lib.locosim_set_terrain_origin.argtypes = [vp, vp]
     lib.locosim_set_body_outputs.restype = ip
     lib.locosim_set_body_outputs.argtypes = [vp, vp, vp]
     lib.locosim_set_contact_outputs.restype = ip
@@ -129,7 +131,7 @@ EXPORTED_SYMBOLS = ["locosim_create", "locosim_destroy", "locosim_last_error", "
                     "locosim_set_reference_outputs", "locosim_create_dataset_bodies", "locosim_inverse",
                     "locosim_create_dataset_inverse", "locosim_dynamics_terms", "locosim_forward", "locosim_state_words",
                     "locosim_save_state", "locosim_load_state", "locosim_max_contacts",
-                    "locosim_set_contact_list_outputs", "locosim_ray"]
+                    "locosim_set_contact_list_outputs", "locosim_ray", "locosim_set_terrain_origin"]
 
 # values per body row of the body outputs (include/locosim.h LS_BODY_DIM): xpos (3), xquat w x y z (4), angular velocity (3),
 # linear velocity of the body-frame origin (3), world frame
@@ -365,6 +367,16 @@ class CudaEngine:
                 self._check_tensor(x, name, shape)
         self._check(self.lib.locosim_set_applied_forces(self.h, _ptr(xfrc), _ptr(qfrc)))
         self._applied = (xfrc, qfrc)
+
+    def set_terrain_origin(self, origin=None):
+        """Register the terrain origin of include/locosim.h (locosim_set_terrain_origin): `origin` float32 cuda [n_envs, 2],
+        the terrain point (x, y) under each env's world origin, read by every later step and query; None = all zeros. The
+        engine keeps a reference to it. Only for a model with a terrain (loco_mujoco_b200.terrain). Register outside of
+        CUDA-graph capture."""
+        if origin is not None:
+            self._check_tensor(origin, "origin", (self.n_envs, 2))
+        self._check(self.lib.locosim_set_terrain_origin(self.h, _ptr(origin)))
+        self._terrain_origin = origin
 
     def set_body_outputs(self, body=None, next_body=None):
         """Register the body outputs of include/locosim.h (MuJoCo's xpos / xquat / body velocity): `body` and `next_body`

@@ -160,6 +160,7 @@ class LocoEnv:
     """Base class of all batched locomotion environments."""
 
     _registered_envs = dict()
+    _terrain_supported = False      # (the robots whose compiled models may carry a terrain: UnitreeA1)
 
     def __init__(self, xml_handles, action_spec, observation_spec, collision_groups=None, gamma=0.99, horizon=1000,
                  n_substeps=10, reward_type=None, reward_params=None, traj_params=None, random_start=True,
@@ -167,7 +168,7 @@ class LocoEnv:
                  use_absorbing_states=True, domain_randomization_config=None, parallel_dom_rand=True,
                  N_worker_per_xml_dom_rand=4, num_envs=None, device="cuda:0", seed=0, env_id_offset=0,
                  compiled_model=None, copy_outputs=True, convex_collisions=True, warps_per_block=None, time_limit=None,
-                 truncate_at_trajectory_end=False, **viewer_params):
+                 truncate_at_trajectory_end=False, terrain=None, **viewer_params):
         if type(xml_handles) != list:
             xml_handles = [xml_handles]
         self._xml_handles = xml_handles
@@ -190,6 +191,19 @@ class LocoEnv:
             self._models = list(compiled_model) if isinstance(compiled_model, (list, tuple)) else [compiled_model]
         else:
             self._models = [mjcf.compile_model(h, timestep=timestep) for h in xml_handles]
+        # terrain: a height field (loco_mujoco_b200.terrain.HeightField) attached to the compiled model as its last geom
+        # (include/locosim.h locosim_set_terrain_origin); UnitreeA1 only
+        if terrain is not None:
+            if domain_randomization_config is not None:
+                # (the randomised parameter pools are built from models without the terrain geom: their rows would not
+                # match the terrain model's)
+                raise NotImplementedError("terrain together with domain_randomization_config is not supported")
+            if not self._terrain_supported:
+                raise NotImplementedError("terrain is implemented for UnitreeA1 only (its floor-colliding geoms are "
+                                          "spheres, capsules, cylinders and boxes), not for %s" % type(self).__name__)
+            from .. import terrain as _terrain
+            self._models = [_terrain.attach(m, terrain) for m in self._models]
+        self._terrain_origin = None
         self._model = self._models[0]
         if timestep is None:
             self._timestep = self._model.opt_timestep
@@ -449,6 +463,8 @@ class LocoEnv:
                 self._engine.set_time_limit(self._max_episode_steps, self._truncate_at_trajectory_end)
             if self._xfrc_applied is not None or self._qfrc_applied is not None:
                 self._engine.set_applied_forces(self._xfrc_applied, self._qfrc_applied)
+            if self._terrain_origin is not None:
+                self._engine.set_terrain_origin(self._terrain_origin)
             if self._body_state is not None:
                 self._engine.set_body_outputs(self._body_state, self._next_body_state)
             if self._contact_wrench is not None:
@@ -490,6 +506,28 @@ class LocoEnv:
         if self._qfrc_applied is None:
             self._qfrc_applied = self._new_applied((self.num_envs, self._model.nv))
         return self._qfrc_applied
+
+    @property
+    def terrain(self):
+        """The height field of this env (loco_mujoco_b200.terrain.HeightField), or None."""
+        return getattr(self._model, "hfield", None)
+
+    @property
+    def terrain_origin(self):
+        """float32 torch tensor [num_envs, 2] on the env's device: per env the terrain point (x, y) that lies under the env's
+        world origin (its reset spot); env i sees the height field translated by -terrain_origin[i]. Write into it in place
+        (also between replays of a captured CUDA graph); every later step and query reads it. Resets do not change it: root
+        x / y restart at 0, so an env restarts on the same terrain point. Allocated zeroed and registered with the engine on
+        first access (touch it before capturing a step in a CUDA graph). Only for an env made with `terrain=`."""
+        if self.terrain is None:
+            raise ValueError("this env has no terrain (LocoEnv.make(..., terrain=HeightField))")
+        if self._terrain_origin is None:
+            import torch
+            eng = self._get_engine()
+            t = torch.zeros((self.num_envs, 2), dtype=torch.float32, device=eng.device)
+            eng.set_terrain_origin(t)
+            self._terrain_origin = t
+        return self._terrain_origin
 
     def _new_applied(self, shape):
         import torch

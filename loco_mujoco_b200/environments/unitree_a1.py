@@ -32,6 +32,7 @@ _TRUNK = ["trunk_tx", "trunk_ty", "trunk_tz", "trunk_list", "trunk_tilt", "trunk
 
 class UnitreeA1(LocoEnv):
     valid_task_confs = ValidTaskConf(tasks=["simple", "hard"], data_types=["real", "perfect"])
+    _terrain_supported = True
 
     def __init__(self, action_mode="torque", setup_random_rot=False, default_target_velocity=0.5, camera_params=None,
                  **kwargs):

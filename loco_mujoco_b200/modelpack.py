@@ -28,35 +28,51 @@ EXTRA_ARRAYS = ["opt_gravity", "body_weldid", "body_dofadr", "body_dofnum", "dof
                 "geom_conaffinity", "site_bodyid", "site_pos", "site_quat"]
 
 
-GEOM_PLANE, GEOM_SPHERE, GEOM_CAPSULE, GEOM_BOX, GEOM_MESH = 0, 2, 3, 6, 7
+GEOM_PLANE, GEOM_HFIELD, GEOM_SPHERE, GEOM_CAPSULE, GEOM_BOX, GEOM_MESH = 0, 1, 2, 3, 6, 7
 PRIMITIVE_PAIRS = {(GEOM_SPHERE, GEOM_SPHERE), (GEOM_SPHERE, GEOM_CAPSULE), (GEOM_CAPSULE, GEOM_CAPSULE), (GEOM_SPHERE, GEOM_BOX)}
 
 
 def convex_pair_mask(m):
     """True for the candidate pairs that go through the general convex routine (mjc_Convex / MPR): everything that is
-    neither a plane pair nor one of the dedicated primitive routines (same rule as csrc/locosim_host.h parse_model)."""
+    neither a plane pair, nor a terrain pair, nor one of the dedicated primitive routines (same rule as
+    csrc/locosim_host.h parse_model)."""
     pg = np.asarray(m.pair_geom).reshape(-1, 2)
     t = np.asarray(m.geom_type)
-    return np.array([t[a] != GEOM_PLANE and (int(t[a]), int(t[b])) not in PRIMITIVE_PAIRS for a, b in pg], dtype=bool)
+    return np.array([t[a] not in (GEOM_PLANE, GEOM_HFIELD) and (int(t[a]), int(t[b])) not in PRIMITIVE_PAIRS for a, b in pg],
+                    dtype=bool).reshape(-1)
+
+
+def terrain_pair_mask(m):
+    """True for the pairs (terrain, g) of a height field (loco_mujoco_b200/terrain.py attach)."""
+    pg = np.asarray(m.pair_geom).reshape(-1, 2)
+    return (np.asarray(m.geom_type)[pg[:, 0]] == GEOM_HFIELD) if len(pg) else np.zeros(0, dtype=bool)
 
 
 def pack(m, convex_pairs=True):
     """Model -> (ints int32[], reals float64[]). convex_pairs=False leaves the general convex (MPR) candidate pairs out of
     the pair table (LocoEnv kwarg `convex_collisions=False`: the round-1 feature set, without bone-bone contacts)."""
     pair_geom = np.asarray(m.pair_geom).reshape(-1, 2)
-    # wire order of the candidate pairs: primitive pairs first, general convex pairs last, model order within each part
-    # (the engine runs a lean bounding-sphere loop over the convex part; contact lists are ordered accordingly)
-    cm = convex_pair_mask(m)
-    pair_geom = pair_geom[~cm] if not convex_pairs else np.concatenate([pair_geom[~cm], pair_geom[cm]])
+    # wire order of the candidate pairs: primitive pairs first, general convex pairs next, the terrain's pairs last, model
+    # order within each part (the engine runs a lean bounding-sphere loop over the convex part and the terrain pass after
+    # it; contact lists are ordered accordingly)
+    cm, tm = convex_pair_mask(m), terrain_pair_mask(m)
+    parts = [pair_geom[~cm & ~tm]] + ([pair_geom[cm]] if convex_pairs else []) + [pair_geom[tm]]
+    pair_geom = np.concatenate(parts)
+    hf = getattr(m, "hfield", None)
     ih = np.zeros(16, dtype=np.int32)
     ih[:11] = [MAGIC, VERSION, m.nbody, m.nv, m.ngeom, m.nu, len(pair_geom), len(m.mesh_vert), m.opt_integrator,
                m.opt_cone, m.opt_iterations]
     rh = np.zeros(16, dtype=np.float64)
     rh[:7] = [m.opt_timestep, m.opt_gravity[0], m.opt_gravity[1], m.opt_gravity[2], m.opt_impratio,
               m.opt_tolerance, m.stat_meaninertia]
+    if hf is not None:      # (header slots MPI_HF_NROW / MPI_HF_NCOL, MPR_HF_SIZE; zeros without a terrain)
+        ih[11:13] = hf.data.shape
+        rh[7:11] = hf.size4
     ints = [ih] + [np.ascontiguousarray(pair_geom if f == "pair_geom" else getattr(m, f), dtype=np.int32).ravel()
                    for f in INT_FIELDS]
     reals = [rh] + [np.ascontiguousarray(getattr(m, f), dtype=np.float64).ravel() for f in REAL_FIELDS]
+    if hf is not None:      # the trailing hfield_data[nrow * ncol]
+        reals.append(np.ascontiguousarray(hf.data, dtype=np.float64).ravel())
     return np.concatenate(ints), np.concatenate(reals)
 
 
